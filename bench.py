@@ -2,6 +2,7 @@
 """bench.py -- MSamples/s of raw I/Q through matched filter -> gate -> tag_decoder.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config cfg2|cfg3|cfg4|cfg5]
+                  [--dump-outputs DIR]
 
 Default workload = BASELINE.json configs[1] ("cfg2"): synthetic 40 kHz-BLF FM0 I/Q @ 2 MS/s, 1000 queries
 (= 1000 inventory-round segments of 16,960 raw samples), 1 tag, per GPU.  One *step* = one pass of the hot path
@@ -34,6 +35,7 @@ sys.path.insert(0, ROOT)
 
 SEG_US = 8480.0
 NBUF = 4          # cfg2: distinct captures cycled through so every step reads data that is not in L2
+DUMP_MAX_SEGMENTS = 65536   # --dump-outputs: larger batches are written as a fixed, seeded sample of segments
 MAX_WINDOWS = 2
 METRIC = "MSamples/s I/Q through gate->tag_decoder"
 BLF = 40000
@@ -58,7 +60,7 @@ def hbm_peak():
             return float(json.load(open(p))["hbm_gbs"]), "measured"
         except Exception:
             pass
-    return 6650.0, "fallback"
+    return 3350.0, "H100 SXM data sheet"
 
 
 class ClockSampler:
@@ -119,6 +121,24 @@ class ClockSampler:
                     reasons.add(nm)
         return {"sm_mhz": float(np.median([r[1] for r in inside])) if inside else None, "sm_max_mhz": self.max_sm,
                 "reasons": sorted(reasons), "samples": len(inside), "window_pad_ms": round(pad * 1e3, 1)}
+
+
+def dump_outputs(out_dir, recs, counts, prefix=""):
+    """Records and window counts as a caller of the timed path receives them, one float64 .npy per field
+    (<prefix>records_<field>.npy [nseg, max_windows(, 16)], <prefix>counts.npy [nseg]).  Batches of more than
+    DUMP_MAX_SEGMENTS segments are sampled (seeded, the same segments every run; <prefix>segment_index.npy)."""
+    os.makedirs(out_dir, exist_ok=True)
+    nseg = counts.size
+    arrays = {}
+    if nseg > DUMP_MAX_SEGMENTS:
+        pick = np.sort(np.random.default_rng(0).choice(nseg, DUMP_MAX_SEGMENTS, replace=False))
+        recs, counts = recs[pick], counts[pick]
+        arrays["segment_index"] = pick
+    arrays["counts"] = counts
+    for f in recs.dtype.names:
+        arrays["records_" + f] = recs[f]
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, prefix + name + ".npy"), np.asarray(a, dtype=np.float64))
 
 
 # ----------------------------------------------------------------------------------------- host topology
@@ -263,7 +283,11 @@ def main():
     ap.add_argument("--generator", default="torch", choices=["torch", "native"],
                     help="workload generator of our arm (cfg2): the torch model (same samples as the CPU reference arm) or the "
                          "library's CUDA closed-loop slot simulator (rfid_b200_sim_capture)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the records and window counts of the last timed step to DIR/*.npy")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl != "ours":
+        ap.error("--dump-outputs applies to --impl ours")
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     if args.steps is None:
         args.steps = 20 if args.config == "cfg2" else 5
@@ -436,6 +460,8 @@ def main():
     gate1 = check(last % nslots, (args.warmup + last) % len(caps))
     if fixed_q == 0:
         assert gate1["epc_crc_ok"] == nseg and gate1["epc_match_truth"] == nseg, "timed step decoded wrongly: %r" % (gate1,)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, *capi.results_to_numpy(res_of(last % nslots), cnt_of(last % nslots), MAX_WINDOWS))
 
     # ------------------------------------------------------------------ sampled bit-exact parity against the oracle
     oracle_par = None
@@ -488,18 +514,8 @@ def main():
         peak, peak_kind = hbm_peak()
         k_avg_ms = k_ms / max(1, k_n)
         achieved = 8.0 * n_raw / (k_avg_ms * 1e-3) / 1e9 if k_n else None
-        traffic, traffic_src = None, None
-        tp = os.path.join(ROOT, "profiles", "traffic.json")   # dram bytes per launch from the committed ncu --set full capture
-        if os.path.exists(tp):
-            try:
-                tj = json.load(open(tp))
-                if tj.get("segments") == nseg and tj.get("config", "cfg2") == args.config:
-                    traffic = tj["dram_bytes_read"] + tj["dram_bytes_write"]
-                    traffic_src = "profiles/traffic.json <- %s (ncu --set full of this kernel at this size; not measured in this run)" % tj.get("report", "?")
-            except Exception:
-                pass
         roofline = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                    "frac": (achieved / peak) if achieved else None, "traffic": traffic, "traffic_source": traffic_src,
+                    "frac": (achieved / peak) if achieved else None, "traffic": None, "traffic_source": None,
                     "kernel": kernel_name(adc_rate, ntaps),
                     "kernel_ms": k_avg_ms, "kernel_launches_timed": k_n, "peak_kind": peak_kind,
                     "algorithmic_bytes_per_launch": 8.0 * n_raw}
@@ -558,6 +574,10 @@ def ingest(args, rank, local_rank):
             segs, recs, counts = rx.ingest_capture_host(iq_np, max_windows=MAX_WINDOWS)
             ts.append(time.perf_counter() - t0)
         t = float(np.median(ts))
+        if args.dump_outputs and kind == "pageable":
+            dump_outputs(args.dump_outputs, recs, counts)
+            np.save(os.path.join(args.dump_outputs, "segments_offset.npy"), segs["offset"].astype(np.float64))
+            np.save(os.path.join(args.dump_outputs, "segments_length.npy"), segs["length"].astype(np.float64))
         ok = int(sum((recs[s, k]["crc_ok"] == 1) for s in range(len(segs)) for k in range(min(int(counts[s]), MAX_WINDOWS)) if recs[s, k]["kind"] == 1))
         rows.append({"host_memory": kind, "seconds_per_call": t, "msamples_per_s": n_raw / t / 1e6, "host_to_device_gbs": 8.0 * n_raw / t / 1e9,
                      "segments_found": int(len(segs)), "epc_crc_ok": ok, "launches_per_call": rx.last_launch_count()})
@@ -606,6 +626,8 @@ def sweep(args, rank, local_rank, world):
         k_ms, k_n = rx.kernel_time(reset=True)
         rx.enable_kernel_timing(False)
         recs, counts = capi.results_to_numpy(res, cnt, MAX_WINDOWS)
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, recs, counts, prefix="adc%d_" % adc)
         ci = (args.warmup + args.steps - 1) % 2
         # parity on a sample of the segments against the oracle at this rate
         pick = np.arange(0, rounds, max(1, rounds // 64))[:64]

@@ -1,4 +1,4 @@
-"""Builds librfid_b200.so (CUDA kernels + C-ABI) in-tree with nvcc for sm_100a."""
+"""Builds librfid_b200.so (CUDA kernels + C-ABI) in-tree with nvcc for sm_90a (H100)."""
 import os
 import shutil
 import subprocess
@@ -10,7 +10,7 @@ SOURCES = ["rfid_b200.cu"]
 import glob
 HEADERS = sorted(os.path.basename(h) for h in glob.glob(os.path.join(CSRC, "*.cuh"))) + ["../../include/rfid_b200.h"]
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               # no FMA contraction: the reference's x86-64 objects contain none (SURVEY.md A.5)
               "-fmad=false",
               "-Xcompiler", "-fPIC,-fvisibility=hidden", "-shared", "-diag-suppress", "550"]

@@ -1,8 +1,8 @@
 """ctypes binding of librfid_b200.so (include/rfid_b200.h) + a thin, torch-aware wrapper.
 
 PyTorch is used only for device memory, streams and (elsewhere) torch.distributed; every
-signal-path operation goes through the C-ABI into the hand-written sm_100a kernels.  There is no
-CPU fallback: constructing `Gen2Rx` without the compiled library or without a B200 raises.
+signal-path operation goes through the C-ABI into the hand-written sm_90a kernels.  There is no
+CPU fallback: constructing `Gen2Rx` without the compiled library or without an H100 raises.
 """
 import ctypes as C
 import os

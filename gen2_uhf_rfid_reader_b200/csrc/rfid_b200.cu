@@ -1,4 +1,4 @@
-// rfid_b200.cu -- C-ABI of the B200-native Gen2 receive chain (see include/rfid_b200.h).
+// rfid_b200.cu -- C-ABI of the H100-native Gen2 receive chain (see include/rfid_b200.h).
 // Host side: context, configuration derivation, launches, host<->device marshalling,
 // READER_STATS reduction.  There is no CPU implementation of the signal path in this
 // library: every entry point that produces samples or decisions launches a kernel.
@@ -79,7 +79,7 @@ struct rfid_b200_ctx {
 
 namespace {
 
-const char* kErrNames[] = {"ok", "invalid argument", "no usable sm_100 CUDA device", "out of memory", "CUDA runtime error",
+const char* kErrNames[] = {"ok", "invalid argument", "no usable sm_90 CUDA device", "out of memory", "CUDA runtime error",
                            "output buffer too small"};
 
 int fail_cuda(rfid_b200_ctx* c, cudaError_t e, const char* what)
@@ -280,7 +280,7 @@ int grow(rfid_b200_ctx* ctx, void** p, size_t* have, size_t need)
 int pack_segments_per_cta(const rfid_b200_ctx* ctx, int nseg)
 {
   if (ctx->pack_g_override > 0) return ctx->pack_g_override;
-  const int sms = ctx->sm_count > 0 ? ctx->sm_count : 148;
+  const int sms = ctx->sm_count > 0 ? ctx->sm_count : 132;
   int g = (nseg + sms - 1) / sms;
   if (g < 1) g = 1;
   if (g > kPMaxSeg) g = kPMaxSeg;
@@ -339,7 +339,7 @@ int rfid_b200_create(const rfid_b200_params* p, rfid_b200_ctx** out)
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || p->device < 0 || p->device >= ndev) { cudaGetLastError(); return RFID_B200_ENODEV; }
   cudaDeviceProp prop;
-  if (cudaGetDeviceProperties(&prop, p->device) != cudaSuccess || prop.major != 10) { cudaGetLastError(); return RFID_B200_ENODEV; }
+  if (cudaGetDeviceProperties(&prop, p->device) != cudaSuccess || prop.major != 9 || prop.minor != 0) { cudaGetLastError(); return RFID_B200_ENODEV; }
   rfid_b200_ctx* ctx = new (std::nothrow) rfid_b200_ctx();
   if (!ctx) return RFID_B200_ENOMEM;
   ctx->params = *p; ctx->cfg = cfg; ctx->device = p->device;
@@ -767,7 +767,7 @@ int launch_mask(rfid_b200_ctx* ctx, const float2* d_iq, size_t n_raw, long long 
 {
   if (n <= 0) return RFID_B200_OK;
   long long blocks = (n + 7) / 8;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > ctx->sm_count * 8) blocks = ctx->sm_count * 8;
   ingest_mask<<<(unsigned)blocks, 256, 0, s>>>(d_iq, n_raw, first_chunk, n, P.tot, P.mask, P.chunk_last, P.chunk_falls);
   CK(cudaGetLastError());
   ctx->last_launches += 1;
@@ -780,7 +780,7 @@ int finish_bursts(rfid_b200_ctx* ctx, long long n_chunks, unsigned int burst_cap
 {
   ingest_scan<<<1, 1024, 0, s>>>(n_chunks, P.chunk_last, P.chunk_falls, P.prev_low, P.falls_before, P.tot);
   long long blocks = (n_chunks + 7) / 8;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > ctx->sm_count * 8) blocks = ctx->sm_count * 8;
   ingest_bursts<<<(unsigned)blocks, 256, 0, s>>>(n_chunks, P.mask, P.prev_low, P.falls_before, sc.gap,
                                                  reinterpret_cast<IngestBurst*>(ctx->d_bursts), burst_cap, P.tot);
   CK(cudaGetLastError());

@@ -1,4 +1,4 @@
-// rx_common.cuh -- shared definitions of the sm_100a Gen2 receive path:
+// rx_common.cuh -- shared definitions of the sm_90a Gen2 receive path:
 // derived configuration, the numerical contract (how each libm/libgcc call the
 // reference makes is evaluated on the device), mbarrier / TMA-bulk PTX wrappers.
 //
@@ -130,15 +130,6 @@ __device__ __forceinline__ float cabsf_quick(float re, float im, bool& risky)
 }
 
 __device__ __forceinline__ float2 c_add(float2 a, float2 b) { return make_float2(f_add(a.x, b.x), f_add(a.y, b.y)); }
-// complex add as ONE packed instruction (sm_100 add.rn.f32x2: two independent IEEE round-to-nearest adds)
-__device__ __forceinline__ float2 c_add2(float2 a, float2 b)
-{
-  unsigned long long ua, ub, ud;
-  ua = ((unsigned long long)__float_as_uint(a.y) << 32) | __float_as_uint(a.x);
-  ub = ((unsigned long long)__float_as_uint(b.y) << 32) | __float_as_uint(b.x);
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(ud) : "l"(ua), "l"(ub));
-  return make_float2(__uint_as_float((unsigned)ud), __uint_as_float((unsigned)(ud >> 32)));
-}
 __device__ __forceinline__ float2 c_sub(float2 a, float2 b) { return make_float2(f_sub(a.x, b.x), f_sub(a.y, b.y)); }
 __device__ __forceinline__ float c_norm(float2 a) { return f_add(f_mul(a.x, a.x), f_mul(a.y, a.y)); }
 // std::real((a - b) * std::conj(h)): (x+iy)(c+id) with d = -h.y, real = x*c - y*d

@@ -352,7 +352,7 @@ __global__ void __launch_bounds__(kSplitThreads, 7) rx_fused_split_kernel(const 
           for (int q = 0; q < 2; q++) {
             float2 b = x[DECIM * q];
 #pragma unroll
-            for (int j = 1; j < DECIM; j++) b = c_add2(b, x[DECIM * q + j]);
+            for (int j = 1; j < DECIM; j++) b = c_add(b, x[DECIM * q + j]);
             w[MFQ - 1 + h + q] = b;
           }
         }
@@ -375,7 +375,7 @@ __global__ void __launch_bounds__(kSplitThreads, 7) rx_fused_split_kernel(const 
         for (int q = 0; q < Q; q++) {
           y[q] = w[q];
 #pragma unroll
-          for (int m = 1; m < MFQ; m++) y[q] = c_add2(y[q], w[q + m]);
+          for (int m = 1; m < MFQ; m++) y[q] = c_add(y[q], w[q + m]);
           a[q] = cabsf_ref(y[q].x, y[q].y);  // gate_impl.cc:130
         }
         {
@@ -468,7 +468,7 @@ __global__ void __launch_bounds__(kSplitThreads, 7) rx_fused_split_kernel(const 
             }
             float2 b = x[0];
   #pragma unroll
-            for (int j = 1; j < DECIM; j++) b = c_add2(b, x[j]);
+            for (int j = 1; j < DECIM; j++) b = c_add(b, x[j]);
             if (MFQ > 0) {
               bhist[MFQ - 1 + t] = b;               // bhist[0 .. MFQ-2] = the last MFQ-1 block sums of the previous tile
               if (t >= kTT - (MFQ - 1)) b_keep[0] = b;  // ... which these threads hand over after the tile
@@ -509,7 +509,7 @@ __global__ void __launch_bounds__(kSplitThreads, 7) rx_fused_split_kernel(const 
               const float2* bp = bhist + t;  // B(n-MFQ+1) .. B(n) are bp[0 .. MFQ-1]
               y = bp[0];
   #pragma unroll
-              for (int m = 1; m < MFQ; m++) y = c_add2(y, bp[m]);
+              for (int m = 1; m < MFQ; m++) y = c_add(y, bp[m]);
             } else {
               int m = n - C.mf_q + 1;
               if (C.mf_rem) {

@@ -390,7 +390,7 @@ __global__ void __launch_bounds__(kPackMaxThreads, 1) rx_pack_kernel(const PackA
             for (int q = 0; q < 2; q++) {
               float2 b = x[DECIM * q];
 #pragma unroll
-              for (int j = 1; j < DECIM; j++) b = c_add2(b, x[DECIM * q + j]);
+              for (int j = 1; j < DECIM; j++) b = c_add(b, x[DECIM * q + j]);
               w[MFQ - 1 + h + q] = b;
             }
           }
@@ -411,7 +411,7 @@ __global__ void __launch_bounds__(kPackMaxThreads, 1) rx_pack_kernel(const PackA
             const int b0 = DECIM * tl - (DECIM - 1) - delta0;
             float2 hb = stage0[b0];
 #pragma unroll
-            for (int j = 1; j < DECIM; j++) hb = c_add2(hb, stage0[b0 + j]);
+            for (int j = 1; j < DECIM; j++) hb = c_add(hb, stage0[b0 + j]);
 #pragma unroll
             for (int m = 0; m < MFQ - 1; m++) halo[m] = make_float2(__shfl_sync(0xffffffffu, hb.x, m), __shfl_sync(0xffffffffu, hb.y, m));
           }
@@ -436,7 +436,7 @@ __global__ void __launch_bounds__(kPackMaxThreads, 1) rx_pack_kernel(const PackA
           for (int q = 0; q < Q; q++) {
             y[q] = w[q];
 #pragma unroll
-            for (int m = 1; m < MFQ; m++) y[q] = c_add2(y[q], w[q + m]);
+            for (int m = 1; m < MFQ; m++) y[q] = c_add(y[q], w[q + m]);
             // outputs past the end of the segment (last, partial tile) are computed from stale shared memory: give them
             // a harmless value so that they cannot push the whole warp onto the rare exact-evaluation paths below
             if (nvalid < kTT && t0 + q >= nvalid) y[q] = make_float2(1.0f, 0.0f);
@@ -744,6 +744,10 @@ __global__ void __launch_bounds__(kPackMaxThreads, 1) rx_pack_kernel(const PackA
             if (lane < 16 && n_e + lane < n16) { er[n_e + lane] = -0.0f; ei[n_e + lane] = -0.0f; }
           }
           if (lane == 0) { B.n_e[s] = n_e; B.trig_n[s] = ntrig; }
+        } else if (have && lane == 0) {
+          // segment over, the CTA's longer segments go on: an empty DC list, so that the chain warp does not replay this
+          // slot's list of five tiles ago (and overwrite dc_val of a window still waiting for its decode)
+          B.n_e[t % kPDS] = 0; B.trig_n[t % kPDS] = 0;
         }
         PP_AT(2)
         __syncwarp();

@@ -3,7 +3,7 @@
  * <nkargas@isc.tuc.gr>, GNU General Public License version 3 or later), because blocks built against it must be
  * drop-in replacements.  The implementation behind the interface is this repository's own.  This file is distributed
  * under the GNU General Public License, version 3 or (at your option) any later version; see LICENSE. */
-/* rfid/api.h -- symbol visibility for the gr::rfid block library (B200 host blocks).
+/* rfid/api.h -- symbol visibility for the gr::rfid block library (H100 host blocks).
  * Same macro name the reference installs (gr-rfid/include/rfid/api.h:27-31) so that
  * application code including <rfid/...> compiles unchanged. */
 #ifndef INCLUDED_RFID_API_H

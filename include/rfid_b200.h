@@ -1,4 +1,4 @@
-/* rfid_b200.h -- C-ABI of the B200-native Gen2 receive/decode chain.
+/* rfid_b200.h -- C-ABI of the H100-native Gen2 receive/decode chain.
  *
  * This is the drop-in boundary: a plain-C shared library (librfid_b200.so) whose
  * entry points are what the reference's three GNU Radio blocks would bind if
@@ -22,7 +22,7 @@
  * torch/C++ types appear in a signature.  Complex samples are interleaved
  * float32 I,Q (GNU Radio gr_complex / the on-disk format of
  * misc/data/file_source_test, apps/reader.py:102).  There is NO CPU fallback:
- * rfid_b200_create() fails with RFID_B200_ENODEV when no sm_100 device is
+ * rfid_b200_create() fails with RFID_B200_ENODEV when no sm_90 device is
  * usable.
  */
 #ifndef RFID_B200_H
@@ -43,7 +43,7 @@ extern "C" {
 enum {
   RFID_B200_OK = 0,
   RFID_B200_EINVAL = -1,   /* bad argument */
-  RFID_B200_ENODEV = -2,   /* no usable sm_100 CUDA device */
+  RFID_B200_ENODEV = -2,   /* no usable sm_90 CUDA device */
   RFID_B200_ENOMEM = -3,   /* host or device allocation failed */
   RFID_B200_ECUDA = -4,    /* CUDA runtime error (see rfid_b200_last_cuda_error) */
   RFID_B200_ECAPACITY = -5 /* caller-provided output buffer too small */

@@ -128,7 +128,7 @@ class FlowLib:
 
 
 def B200Flow():
-    """the A/B harness around THIS repo's host blocks (needs a B200 at run time)"""
+    """the A/B harness around THIS repo's host blocks (needs an H100 at run time)"""
     path = os.path.join(HERE, "libgen2flow_b200.so")
     if not os.path.exists(path):
         raise FileNotFoundError(path + " (make -C oracle flow_b200)")

@@ -12,7 +12,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu)")
 
 
 @pytest.fixture(scope="session")
@@ -36,12 +36,11 @@ def oracle():
 
 
 @pytest.fixture(scope="session")
-def ref_flow():
-    """oracle/_ref: the reference's own blocks compiled unchanged (skips when it was not built)."""
-    from oracle import refflow
-    if not refflow.ref_available(0):
-        pytest.skip("oracle/_ref not built (needs /root/reference at build time)")
-    return refflow.RefFlow(0)
+def ref_outputs():
+    """What the reference's own blocks (oracle/_ref) computed on the inputs of the reference comparisons
+    (tests/golden/make_golden.py: reference_outputs)."""
+    with np.load(os.path.join(GOLDEN, "reference_outputs.npz")) as z:
+        return {k: z[k] for k in z.files}
 
 
 def records_equal(a, b):

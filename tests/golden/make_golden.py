@@ -11,6 +11,8 @@
   cfg1_ref_records.npy      rfid_b200_window_result records produced by oracle/_ref (the reference's own
                             blocks) on file_source_test; cfg1_ref_stats.json the READER_STATS + print_results text
   cfg1_q4_*.                the same with FIXED_Q = 4
+  reference_outputs.npz     everything else the tests compare with the reference's own blocks (see
+                            reference_outputs()), so that the suite runs where the reference is absent
 """
 import json
 import lzma
@@ -85,7 +87,47 @@ def main():
                    "n_epc_correct": s.n_epc_correct, "tag_reads": {str(k): v for k, v in s.tag_map().items()},
                    "n_windows": r["n_windows"]},
                   open(os.path.join(HERE, tag + "_ref_stats.json"), "w"), indent=1)
+    reference_outputs(iq)
     print("golden regenerated:", sorted(os.listdir(HERE)))
+
+
+# inputs of the comparisons with the reference; the tests rebuild the same inputs
+SYNTH_KW = [dict(n_tags=1), dict(n_tags=0), dict(n_tags=6, fixed_q=2), dict(n_tags=1, noise_sigma=0.02)]
+
+
+def reader_script_bits():
+    return np.random.default_rng(3).integers(0, 2, size=(9, 16)).astype(np.float32)
+
+
+def tx_synth_rn16s():
+    rn16s = np.random.default_rng(11).integers(0, 65536, size=12)
+    rn16s[0], rn16s[1] = 0x0579, 0xFFFF     # first RN16 of the author's TX capture; all data-1
+    return rn16s
+
+
+def reference_outputs(iq):
+    """oracle/_ref run on the inputs of the reference comparisons in tests/ -> reference_outputs.npz"""
+    from gen2_uhf_rfid_reader_b200 import synth
+    from oracle.refflow import RefFlow
+    ref, ref4 = RefFlow(0), RefFlow(4)
+    out = {}
+    r = ref.run_stream(iq, want_tx=True)
+    out["cfg1_tx"] = r["tx"]
+    for chunk in (257, 4096, 100000):
+        out["cfg1_records_chunk%d" % chunk] = ref.run_stream(iq, chunk=chunk)["records"]
+    for i, kw in enumerate(SYNTH_KW):
+        cap = synth.make_capture(48, seed=21, **kw)
+        out["synth48_%d_records" % i], out["synth48_%d_counts" % i], _ = \
+            ref.run_segments(cap["iq"].numpy(), cap["segments"], max_per_seg=4)
+    cap = synth.make_capture(40, seed=5)
+    out["synth40_records"], out["synth40_counts"], _ = ref.run_segments(cap["iq"].numpy(), cap["segments"], max_per_seg=4)
+    out["reader_script_tx"], out["reader_script_nq"] = ref.reader_script(reader_script_bits())
+    rn16s = tx_synth_rn16s()
+    bits = ((rn16s[:, None] >> np.arange(15, -1, -1)[None, :]) & 1).astype(np.float32)
+    for dac_rate in (1000000, 2000000):
+        out["tx_synth_%d" % dac_rate], out["tx_synth_%d_nq" % dac_rate] = ref.reader_script(bits, dac_rate=dac_rate)
+    out["tx_synth_q4"], _ = ref4.reader_script(np.zeros((2, 16), dtype=np.float32))
+    np.savez_compressed(os.path.join(HERE, "reference_outputs.npz"), **out)
 
 
 if __name__ == "__main__":

@@ -95,7 +95,7 @@ def test_gather_records_world2_gloo():
         assert got[f].tobytes() == recs[f].tobytes(), f
 
 
-def test_reader_block_matches_reference_sample_for_sample(ref_flow):
+def test_reader_block_matches_reference_sample_for_sample(ref_outputs):
     """this repo's reader block (Gen2 logic + PIE generator, host C++) vs the reference's, scripted on CPU:
     START, Query/QueryRep alternating, ACK(RN16), CW -- identical TX envelope and query count"""
     from oracle import refflow
@@ -104,7 +104,7 @@ def test_reader_block_matches_reference_sample_for_sample(ref_flow):
     except FileNotFoundError:
         pytest.skip("oracle/libgen2flow_b200.so not built")
     bits = np.random.default_rng(3).integers(0, 2, size=(9, 16)).astype(np.float32)
-    a, na = ref_flow.reader_script(bits)
+    a, na = ref_outputs["reader_script_tx"], ref_outputs["reader_script_nq"]
     b, nb = mine.reader_script(bits)
     assert na == nb == 9
     assert a.size == b.size and np.array_equal(a, b)

@@ -1,7 +1,8 @@
 """CPU tests: the oracle is pinned to the reference's golden vectors and to the reference's own code.
 
 Golden material (SURVEY.md section 4 / Appendix B): README.md:46-53 expected output, the RN16s the reference
-author's run decoded (recovered from misc/data/file_sink), and records produced here by oracle/_ref.
+author's run decoded (recovered from misc/data/file_sink), and what oracle/_ref (the reference's own blocks under
+our scheduler) produced, stored by tests/golden/make_golden.py.
 """
 import json
 import os
@@ -22,11 +23,10 @@ def _readme_numbers():
             "tag": int(g(r"Tag ID : (\w+)"), 16), "reads": int(g(r"Num of reads : (\d+)"))}
 
 
-def test_reference_reproduces_readme(ref_flow, cfg1_iq):
+def test_reference_reproduces_readme():
     """the compiled reference + our scheduler print the README block (README.md:48-53)"""
-    r = ref_flow.run_stream(cfg1_iq)
     exp = _readme_numbers()
-    t = r["text"]
+    t = json.load(open(os.path.join(GOLDEN, "cfg1_ref_stats.json")))["text"]
     assert "queryreps sent : %d" % exp["sent"] in t
     assert "Inventory round : %d" % exp["round"] in t
     assert "decoded EPC : %d" % exp["epc"] in t
@@ -35,10 +35,9 @@ def test_reference_reproduces_readme(ref_flow, cfg1_iq):
     assert exp == {"sent": 71, "round": 72, "epc": 70, "unique": 1, "tag": 0x27, "reads": 70}
 
 
-def test_reference_chunk_size_independent(ref_flow, cfg1_iq, cfg1_golden):
+def test_reference_chunk_size_independent(ref_outputs, cfg1_golden):
     for chunk in (257, 4096, 100000):
-        r = ref_flow.run_stream(cfg1_iq, chunk=chunk)
-        assert not records_equal(r["records"], cfg1_golden), chunk
+        assert not records_equal(ref_outputs["cfg1_records_chunk%d" % chunk], cfg1_golden), chunk
 
 
 def test_golden_rn16_match_author_run(cfg1_golden):
@@ -51,18 +50,18 @@ def test_golden_rn16_match_author_run(cfg1_golden):
     assert all(a.startswith("01") for a in cmds["acks"])
 
 
-def test_reference_tx_matches_author_run(ref_flow, cfg1_iq):
+def test_reference_tx_matches_author_run(ref_outputs):
     """the reader block's own TX envelope (driven by our scheduler) = the committed file_sink, command by command"""
     import sys
     sys.path.insert(0, GOLDEN)
     from make_golden import decode_pie
-    r = ref_flow.run_stream(cfg1_iq, want_tx=True)
-    cmds = decode_pie(r["tx"])
+    tx = ref_outputs["cfg1_tx"]
+    cmds = decode_pie(tx)
     gold = json.load(open(os.path.join(GOLDEN, "file_sink_commands.json")))
     q = [b for k, b in cmds if k == "preamble"]
     a = [b for k, b in cmds if k == "framesync"]
     assert q[:72] == gold["queries"] and a[:71] == gold["acks"]
-    assert abs(len(r["tx"]) - 539864) <= 8  # flowgraph stop point differs by a few samples
+    assert abs(len(tx) - 539864) <= 8  # flowgraph stop point differs by a few samples
 
 
 def test_restatement_equals_reference_on_cfg1(oracle, cfg1_iq, cfg1_golden):
@@ -90,11 +89,15 @@ def test_stats_reduction_matches_reference(oracle, cfg1_golden):
         (g4["n_queries_sent"], g4["cur_inventory_round"], g4["cur_slot_number"], g4["n_epc_correct"])
 
 
-@pytest.mark.parametrize("kw", [dict(n_tags=1), dict(n_tags=0), dict(n_tags=6, fixed_q=2), dict(n_tags=1, noise_sigma=0.02)])
-def test_restatement_equals_reference_on_synthetic(oracle, ref_flow, kw):
+SYNTH_KW = [dict(n_tags=1), dict(n_tags=0), dict(n_tags=6, fixed_q=2), dict(n_tags=1, noise_sigma=0.02)]
+
+
+@pytest.mark.parametrize("kw", SYNTH_KW)
+def test_restatement_equals_reference_on_synthetic(oracle, ref_outputs, kw):
     cap = synth.make_capture(48, seed=21, **kw)
     iq = cap["iq"].numpy()
-    rr, rc, _ = ref_flow.run_segments(iq, cap["segments"], max_per_seg=4)
+    i = SYNTH_KW.index(kw)   # same order as make_golden.SYNTH_KW
+    rr, rc = ref_outputs["synth48_%d_records" % i], ref_outputs["synth48_%d_counts" % i]
     orr, oc, _ = oracle.decode_segments(iq, cap["segments"], max_per_seg=4)
     assert (rc == oc).all()
     assert not records_equal(rr, orr)

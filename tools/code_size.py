@@ -3,7 +3,7 @@
 import os, re, shutil, subprocess, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SRC = os.path.join(ROOT, "gen2_uhf_rfid_reader_b200", "csrc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-fmad=false", "-cubin"]
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-fmad=false", "-cubin"]
 variants = {"full": None, "no workers": "if (role >= 2 && role < 2 + kSWWarps) {", "no chain": "} else if (role == 0) {",
             "no control": "} else if (role == 1) {", "no decoder": "DECODER"}
 for name, pat in variants.items():

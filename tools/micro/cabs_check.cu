@@ -1,5 +1,5 @@
 // Developer aid: cabsf_quick (+ its risky flag) against cabsf_ref on the GPU: random inputs over many magnitude
-// ranges, the rounding-boundary neighbourhoods, zeros.  Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -fmad=false
+// ranges, the rounding-boundary neighbourhoods, zeros.  Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -fmad=false
 //   -o tools/micro/cabs_check tools/micro/cabs_check.cu ; run on the GPU box.  Prints mismatches (must be 0) and the risky rate.
 #include <cstdio>
 #include <cstdint>

@@ -5,7 +5,7 @@
 set -e
 cd "$(dirname "$0")/.."
 CS=gen2_uhf_rfid_reader_b200/csrc
-FLAGS="-gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 -fmad=false -Xcompiler -fPIC,-fvisibility=hidden -shared -diag-suppress 550,177"
+FLAGS="-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -fmad=false -Xcompiler -fPIC,-fvisibility=hidden -shared -diag-suppress 550,177"
 mkdir -p gpurun_in
 if [ "$1" = build ]; then
   shift
