@@ -132,6 +132,11 @@ class Gen2Rx:
         self.params = params if params is not None else default_params(**kw)
         h = C.c_void_p()
         rc = self.lib.rfid_b200_create(C.byref(self.params), C.byref(h))
+        if rc == abi.EINVAL:
+            raise RfidB200Error("rfid_b200_create: %s: the parameters are out of range, or the configuration is not well "
+                                "defined (at adc_rate=%d, decim=%d the reference decoder reads past the end of its windows; "
+                                "see rfid_b200.h)" % (self.lib.rfid_b200_strerror(rc).decode(), self.params.adc_rate,
+                                                      self.params.decim))
         if rc != 0:
             raise RfidB200Error("rfid_b200_create: %s" % self.lib.rfid_b200_strerror(rc).decode())
         self.h = h

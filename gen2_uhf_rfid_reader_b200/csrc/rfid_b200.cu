@@ -100,6 +100,36 @@ int next_pow2(int v)
   return p;
 }
 
+// The reference's decoder takes every read index from the float n_samples_TAG_BIT, while the gate sizes its windows
+// from the truncated integer (gate_impl.cc:115,121).  Where the two differ too much the EPC symbol-period search and bit
+// decisions read past the end of the window (undefined behaviour in the reference, so there is no answer to reproduce),
+// and an RN16 window can end before its 32 half-bits, after which the reference no longer alternates RN16 / EPC windows.
+// A configuration is well defined when, for every sync index tag_sync can return, every read of the decoder stays
+// inside its window and the RN16 loop reaches 32 half-bits.  Same expressions and types as tag_decoder_impl.cc.
+bool well_defined(const RxConfig& c)
+{
+  const float n = c.n_tag_bit_f;
+  for (int s = 0; s < c.sync_range; s++) {
+    for (int j = 0; j < 2 * kTagPreambleBits; j++)  // tag_sync's correlation and h_est (:92,103)
+      if ((int)(s + j * n / 2) >= c.len_rn16) return false;
+    const int index = (int)(s + kTagPreambleBits * n + n / 2);  // :107
+    int half_bits = 0;
+    for (float j = (float)index; j < c.len_rn16; j += n / 2) {   // :237-253
+      if ((int)std::round(j) >= c.len_rn16) return false;
+      if (++half_bits == 2 * (kRN16Bits - 1)) break;
+    }
+    if (half_bits != 2 * (kRN16Bits - 1)) return false;
+    for (int t = 0; t < 20; t++) {
+      const float T = c.t_min + t * (c.t_max - c.t_min) / (20 - 1);  // :161,166
+      for (int i = 0; i < 256; i++)
+        if ((int)(i * T + index) >= c.len_epc) return false;
+      for (int j = 0; j < 128; j++)  // :173
+        if ((int)(j * (2 * T) + index) >= c.len_epc || (int)(j * 2 * T + T + index) >= c.len_epc) return false;
+    }
+  }
+  return true;
+}
+
 // Derived counts with the reference's own expression order and types
 // (gate_impl.cc:48-53,115,121; tag_decoder_impl.cc:60,85,151-152; global_vars.h:110-111).
 int derive_config(const rfid_b200_params& p, RxConfig& c)
@@ -138,6 +168,7 @@ int derive_config(const rfid_b200_params& p, RxConfig& c)
   }
   if (c.win_length < 1 || c.dc_length < 1 || c.n_tag_bit_i < 1 || c.win_length > kMaxWinLen || c.dc_length > kMaxDcLen)
     return RFID_B200_EINVAL;
+  if (!well_defined(c)) return RFID_B200_EINVAL;
   return RFID_B200_OK;
 }
 

@@ -114,7 +114,19 @@ RFID_B200_API void rfid_b200_default_params(rfid_b200_params* p);
 
 /* Context: one per block instance (block mode) or per decode stream (capture mode).
  * Replaces the constructors gate_impl.cc:41-70 / tag_decoder_impl.cc:50-62 and the
- * process-global reader_state (global_vars.cc:34-54). */
+ * process-global reader_state (global_vars.cc:34-54).
+ *
+ * Fails with RFID_B200_EINVAL, before looking for a device, when the configuration
+ * is not well defined: the reference decoder takes its read indices from the float
+ * samples-per-tag-bit but the gate sizes its windows from the truncated integer, so
+ * at most rates whose tag bit is not a whole number of decimated samples the EPC
+ * symbol-period search reads past the end of its window (undefined behaviour in the
+ * reference) or an RN16 window ends before its 32 half-bits.  Well defined are the
+ * rates where, for every sync index, all of the decoder's reads stay inside the
+ * window.  With decimation 5 these are 314 of the 7001 rates on the 1 kHz grid from
+ * 1 to 8 MS/s: every multiple of 200 kHz but 5.8 MS/s (where the gate's double
+ * product 25 * 1.16 truncates to 28 samples per tag bit and the decoder's float
+ * is 29), and some rates in between. */
 RFID_B200_API int rfid_b200_create(const rfid_b200_params* p, rfid_b200_ctx** out);
 RFID_B200_API void rfid_b200_destroy(rfid_b200_ctx* ctx);
 

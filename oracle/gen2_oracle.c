@@ -22,6 +22,48 @@ enum {
 static const int O_TAG_PREAMBLE[12] = {1, 1, 0, 1, 0, 0, 1, 0, 0, 0, 1, 1}; /* global_vars.h:136 */
 static const float O_THRESH_FRACTION = 0.75f;                               /* global_vars.h:139 */
 
+/* Does tag_decoder_impl.cc stay inside its windows?  The decoder's indices come from the float n_samples_TAG_BIT, the
+ * window lengths from its truncation (gate_impl.cc:115,121).  For each sync index tag_sync can return (i < 1.5 n, :85),
+ * the largest index of every read is formed with the expressions below (the same ones o_tag_sync and
+ * gen2_oracle_decode_window evaluate) and compared with the window it reads. */
+static int o_defined(const gen2_oracle_cfg* c)
+{
+  const float n = c->n_tag_bit_f;
+  if (c->n_tag_bit_i < 1) return 0;
+  for (int i = 0; i < 1.5 * n; i++) {
+    int reach = 0;
+    for (int j = 0; j < 2 * O_TAG_PREAMBLE_BITS; j++) { /* :92; h_est's taps (:103) are among these */
+      int k = (int)(i + j * n / 2);
+      if (k > reach) reach = k;
+    }
+    if (reach >= c->len_rn16) return 0;
+    int index = (int)(i + O_TAG_PREAMBLE_BITS * n + n / 2); /* :107 */
+    int half_bits = 0;                                      /* :237-253 */
+    for (float j = (float)index; j < c->len_rn16; j += n / 2) {
+      if ((int)round(j) >= c->len_rn16) return 0;
+      half_bits++;
+      if (half_bits == 2 * (O_RN16_BITS - 1)) break;
+    }
+    if (half_bits != 2 * (O_RN16_BITS - 1)) return 0;
+    float min_val = (float)(n / 2.0 - n / 2.0 / 100), max_val = (float)(n / 2.0 + n / 2.0 / 100); /* :151-152 */
+    reach = 0;
+    for (int t = 0; t < 20; t++) {
+      float step = min_val + t * (max_val - min_val) / (20 - 1); /* :161 and T, :166 */
+      for (int q = 0; q < 256; q++) {
+        int p = (int)(q * step + index);
+        if (p > reach) reach = p;
+      }
+      for (int q = 0; q < 128; q++) { /* :173 */
+        int a = (int)(q * (2 * step) + index), b = (int)(q * 2 * step + step + index);
+        if (a > reach) reach = a;
+        if (b > reach) reach = b;
+      }
+    }
+    if (reach >= c->len_epc) return 0;
+  }
+  return 1;
+}
+
 void gen2_oracle_make_cfg(const rfid_b200_params* p, gen2_oracle_cfg* c)
 {
   memset(c, 0, sizeof(*c));
@@ -46,6 +88,7 @@ void gen2_oracle_make_cfg(const rfid_b200_params* p, gen2_oracle_cfg* c)
   c->fixed_q = p->fixed_q;
   c->max_queries = p->max_queries;
   c->max_tags = p->max_tags;
+  c->defined = o_defined(c);
 }
 
 size_t gen2_oracle_mf(const float* x, size_t n_in, int ntaps, int decim, float* y)

@@ -43,6 +43,8 @@ typedef struct gen2_oracle_cfg {
   int len_epc;       /* (129+6)*n + 2n                  gate_impl.cc:115 */
   int fixed_q, max_queries, max_tags;
   int adc_rate, decim, ntaps;
+  int defined;       /* 1: every read of tag_decoder_impl.cc stays inside its window and an RN16 window holds its 32
+                      * half-bits, for every sync index; 0: the reference has no defined output to restate */
 } gen2_oracle_cfg;
 
 GEN2_ORACLE_API void gen2_oracle_make_cfg(const rfid_b200_params* p, gen2_oracle_cfg* c);

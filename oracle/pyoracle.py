@@ -18,7 +18,8 @@ class OracleCfg(C.Structure):
     _fields_ = [("fs_dec", C.c_int), ("n_T1", C.c_int), ("n_PW", C.c_int), ("n_tag_bit_i", C.c_int),
                 ("n_tag_bit_f", C.c_float), ("win_length", C.c_int), ("dc_length", C.c_int),
                 ("len_rn16", C.c_int), ("len_epc", C.c_int), ("fixed_q", C.c_int), ("max_queries", C.c_int),
-                ("max_tags", C.c_int), ("adc_rate", C.c_int), ("decim", C.c_int), ("ntaps", C.c_int)]
+                ("max_tags", C.c_int), ("adc_rate", C.c_int), ("decim", C.c_int), ("ntaps", C.c_int),
+                ("defined", C.c_int)]
 
 
 def build():
@@ -30,6 +31,15 @@ def default_params(adc_rate=2000000, decim=5, ntaps=25, fixed_q=0, max_queries=1
                       max_tags=max_tags, device=0, reserved=0)
 
 
+def derive_cfg(params=None, **kw):
+    """the derived constants (OracleCfg) of a configuration, including whether it is defined; never raises"""
+    if not os.path.exists(LIB):
+        build()
+    cfg = OracleCfg()
+    C.CDLL(LIB).gen2_oracle_make_cfg(C.byref(params if params is not None else default_params(**kw)), C.byref(cfg))
+    return cfg
+
+
 class Oracle:
     def __init__(self, params=None, **kw):
         if not os.path.exists(LIB):
@@ -38,6 +48,10 @@ class Oracle:
         self.params = params if params is not None else default_params(**kw)
         self.cfg = OracleCfg()
         L.gen2_oracle_make_cfg(C.byref(self.params), C.byref(self.cfg))
+        if not self.cfg.defined:
+            raise ValueError("adc_rate=%d, decim=%d: the reference decoder reads past the end of its windows at this "
+                             "configuration, so there is no defined output to restate" % (self.params.adc_rate,
+                                                                                          self.params.decim))
         L.gen2_oracle_gate.restype = C.c_int
         L.gen2_oracle_decode_decimated.restype = C.c_int
         L.gen2_oracle_decode_segments.restype = C.c_int

@@ -13,6 +13,8 @@
   cfg1_q4_*.                the same with FIXED_Q = 4
   reference_outputs.npz     everything else the tests compare with the reference's own blocks (see
                             reference_outputs()), so that the suite runs where the reference is absent
+  reference_rates.npz       oracle/_ref records and counts at other sample rates (rate_outputs(); regenerate it
+                            alone with `make_golden.py rates`)
 """
 import json
 import lzma
@@ -88,6 +90,7 @@ def main():
                    "n_windows": r["n_windows"]},
                   open(os.path.join(HERE, tag + "_ref_stats.json"), "w"), indent=1)
     reference_outputs(iq)
+    rate_outputs()
     print("golden regenerated:", sorted(os.listdir(HERE)))
 
 
@@ -130,5 +133,49 @@ def reference_outputs(iq):
     np.savez_compressed(os.path.join(HERE, "reference_outputs.npz"), **out)
 
 
+# (adc rate, taps) of the comparisons at other sample rates, one or more per kernel the library picks there:
+# rx_fused_split_kernel<5,0> / <5,5> at 1.0 MS/s, rx_pack_kernel at 1.2 MS/s, rx_fused_split_kernel<5,5> at 1.4-2.4 MS/s,
+# rx_fused_kernel from 2.6 MS/s up.  Every one is a well-defined rate (tests/rate_rule.py).
+RATES = [(1000000, 12), (1000000, 25), (1200000, 25), (1400000, 25), (1800000, 25), (2200000, 25), (2400000, 25),
+         (2600000, 25), (3000000, 25), (5000000, 25), (4000000, 50), (8000000, 100)]
+# capture variants: name -> make_capture keywords ("quiet": noise- and drift-free, which makes exact ties for the
+# decoder's first-maximum rules)
+RATE_VARIANTS = {"default": dict(), "quiet": dict(noise_sigma=0.0, clock_ppm_pct=0.0), "notag": dict(n_tags=0),
+                 "noisy": dict(noise_sigma=0.02)}
+RATE_Q4 = dict(fixed_q=4, n_tags=8)      # through the FIXED_Q = 4 build, at these rates only
+RATE_Q4_RATES = (1200000, 2400000)
+
+
+def rate_cases():
+    """(key, adc_rate, ntaps, make_capture keywords) of every stored comparison at other rates"""
+    out = []
+    for adc, ntaps in RATES:
+        for name, kw in RATE_VARIANTS.items():
+            out.append(("r%d_t%d_%s" % (adc, ntaps, name), adc, ntaps, kw))
+        if adc in RATE_Q4_RATES:
+            out.append(("r%d_t%d_q4" % (adc, ntaps), adc, ntaps, RATE_Q4))
+    return out
+
+
+def rate_capture(adc, kw):
+    from gen2_uhf_rfid_reader_b200 import synth
+    return synth.make_capture(24, seed=31, adc_rate=adc, **kw)
+
+
+def rate_outputs():
+    """oracle/_ref on 24 segments at each rate and variant of rate_cases() -> reference_rates.npz"""
+    from oracle.refflow import RefFlow
+    ref = {0: RefFlow(0), 4: RefFlow(4)}
+    out = {}
+    for key, adc, ntaps, kw in rate_cases():
+        cap = rate_capture(adc, kw)
+        out[key + "_records"], out[key + "_counts"], _ = ref[kw.get("fixed_q", 0)].run_segments(
+            cap["iq"].numpy(), cap["segments"], adc_rate=adc, ntaps=ntaps, max_per_seg=4)
+    np.savez_compressed(os.path.join(HERE, "reference_rates.npz"), **out)
+
+
 if __name__ == "__main__":
-    main()
+    if sys.argv[1:] == ["rates"]:
+        rate_outputs()
+    else:
+        main()

@@ -119,3 +119,24 @@ def test_sass_of_the_new_kernels_is_present():
     out = subprocess.check_output(["cuobjdump", "-sass", capi.LIB], text=True)
     for k in ("ingest_mask", "ingest_scan", "ingest_bursts", "tx_synth_kernel", "sim_slot_kernel", "rx_fused_split_kernel", "rx_pack_kernel"):
         assert k in out, k
+
+
+def test_create_refuses_rates_that_are_not_well_defined():
+    """rfid_b200_create checks, before it looks for a device, that the reference decoder stays inside its windows at the
+    configured rate (csrc/rfid_b200.cu: well_defined); against the independent numpy evaluation on the 1 kHz grid from
+    1 to 8 MS/s: EINVAL exactly where the configuration is not well defined"""
+    import rate_rule
+    lib = capi.load_library()
+    want = rate_rule.well_defined(rate_rule.GRID)
+    h = C.c_void_p()
+    rc = []
+    for r in rate_rule.GRID:
+        rc.append(lib.rfid_b200_create(C.byref(capi.default_params(adc_rate=int(r))), C.byref(h)))
+        if rc[-1] == abi.OK:     # a GPU is present
+            lib.rfid_b200_destroy(h)
+    rc = np.array(rc)
+    assert (rc[~want] == abi.EINVAL).all(), rate_rule.GRID[~want & (rc != abi.EINVAL)][:10]
+    assert set(rc[want].tolist()) <= {abi.ENODEV, abi.OK}, rate_rule.GRID[want & (rc == abi.EINVAL)][:10]
+    for adc in (1_520_000, 1_360_000, 5_800_000):
+        with pytest.raises(capi.RfidB200Error, match="not well defined"):
+            capi.Gen2Rx(adc_rate=adc)

@@ -7,12 +7,17 @@ our scheduler) produced, stored by tests/golden/make_golden.py.
 import json
 import os
 import re
+import sys
 
 import numpy as np
 import pytest
 
 from conftest import GOLDEN, records_equal
 from gen2_uhf_rfid_reader_b200 import abi, synth
+
+sys.path.insert(0, GOLDEN)
+from make_golden import RATE_VARIANTS, rate_capture, rate_cases  # noqa: E402
+import rate_rule  # noqa: E402
 
 
 def _readme_numbers():
@@ -188,3 +193,100 @@ def test_empty_and_short_segments(oracle):
     segs = abi.make_segments([0, 5, 100, 0], [0, 3, 4, 700])
     recs, counts, _ = oracle.decode_segments(iq, segs, max_per_seg=2)
     assert counts.tolist() == [0, 0, 0, 0]
+
+
+# ------------------------------------------------------------------ other sample rates
+@pytest.fixture(scope="session")
+def ref_rates():
+    """What the reference's own blocks computed at other sample rates (tests/golden/make_golden.py: rate_outputs)."""
+    with np.load(os.path.join(GOLDEN, "reference_rates.npz")) as z:
+        return {k: z[k] for k in z.files}
+
+
+@pytest.mark.parametrize("case", rate_cases(), ids=[c[0] for c in rate_cases()])
+def test_restatement_equals_reference_at_other_rates(ref_rates, case):
+    """the restatement against the reference's compiled blocks at every stored rate, tap count and capture variant,
+    every field of every record and the window counts"""
+    from oracle.pyoracle import Oracle
+    key, adc, ntaps, kw = case
+    cap = rate_capture(adc, kw)
+    orr, oc, _ = Oracle(adc_rate=adc, ntaps=ntaps, fixed_q=kw.get("fixed_q", 0)).decode_segments(
+        cap["iq"].numpy(), cap["segments"], max_per_seg=4)
+    assert oc.tolist() == ref_rates[key + "_counts"].tolist()
+    assert not records_equal(orr, ref_rates[key + "_records"])
+    assert oc.sum() >= 8
+
+
+def _sync_correlation(win, n):
+    """tag_sync's |corr|^2 for every i < 1.5 n (tag_decoder_impl.cc:85-95), float32 in the reference's order"""
+    i = np.arange(int(np.ceil(1.5 * float(n))))
+    cr, ci = np.zeros(i.size, np.float32), np.zeros(i.size, np.float32)
+    for j, p in enumerate((1, 1, 0, 1, 0, 0, 1, 0, 0, 0, 1, 1)):
+        k = (i.astype(np.float32) + np.float32(j) * n / np.float32(2)).astype(np.int64)
+        if p:
+            cr, ci = cr + win[k].real, ci + win[k].imag
+    return cr * cr + ci * ci
+
+
+def _period_energies(win, n, index):
+    """tag_detection_EPC's energy[t] and half-periods (tag_decoder_impl.cc:151-166), float32 in the reference's order"""
+    n64 = np.float64(n)
+    lo, hi = np.float32(n64 / 2.0 - n64 / 2.0 / 100), np.float32(n64 / 2.0 + n64 / 2.0 / 100)
+    steps = lo + np.arange(20, dtype=np.float32) * (hi - lo) / np.float32(19)
+    m2 = win.real * win.real + win.imag * win.imag
+    e = np.zeros(20, np.float32)
+    for q in range(256):
+        e = e + m2[(np.float32(q) * steps + np.float32(index)).astype(np.int64)]
+    return e, steps
+
+
+def test_quiet_captures_tie_the_first_maximum_rules():
+    """The noise- and drift-free captures of the rate comparisons exist to produce exact ties where the reference keeps
+    the first maximum (tag_sync's strict '>', std::max_element).  Recompute both searches in numpy float32 on the
+    gate's windows: the first maximum is the restatement's sync_index and T, and ties do occur, in both searches."""
+    from oracle.pyoracle import Oracle
+    sync_ties, t_ties = {}, {}
+    for key, adc, ntaps, kw in rate_cases():
+        if kw is not RATE_VARIANTS["quiet"]:
+            continue
+        o = Oracle(adc_rate=adc, ntaps=ntaps)
+        n = np.float32(o.cfg.n_tag_bit_f)
+        cap = rate_capture(adc, kw)
+        iq = cap["iq"].numpy()
+        sync_ties[adc, ntaps] = t_ties[adc, ntaps] = 0
+        for s in cap["segments"]:
+            y = o.mf(iq[int(s["offset"]):int(s["offset"]) + int(s["length"])])
+            wins = o.gate(y, want_windows=True)["windows"]
+            recs, _ = o.decode_decimated(y)
+            for k, r in enumerate(recs):
+                w = wins[k, :r["length"]]
+                c = _sync_correlation(w, n)
+                first = int(np.argmax(c))
+                assert first == r["sync_index"] and c[first] == r["score"], (key, k)
+                sync_ties[adc, ntaps] += int((c == c[first]).sum() > 1)
+                if r["kind"] == abi.EPC:
+                    index = int(np.float32(first) + np.float32(6) * n + n / np.float32(2))
+                    e, steps = _period_energies(w, n, index)
+                    t = int(np.argmax(e))
+                    assert steps[t] == r["T"], (key, k)
+                    t_ties[adc, ntaps] += int((e == e[t]).sum() > 1)
+    assert sum(v > 0 for v in sync_ties.values()) >= 4, sync_ties
+    assert sum(t_ties.values()) > 0, t_ties
+
+
+def test_well_defined_rates_restatement_agrees_with_numpy():
+    """gen2_oracle_make_cfg's `defined` against the independent numpy evaluation, on the 1 kHz grid from 1 to 8 MS/s;
+    the restatement refuses an undefined configuration instead of reading past its window"""
+    from oracle.pyoracle import Oracle, derive_cfg
+    want = rate_rule.well_defined(rate_rule.GRID)
+    got = np.array([derive_cfg(adc_rate=int(r)).defined for r in rate_rule.GRID], dtype=bool)
+    assert (got == want).all(), rate_rule.GRID[got != want][:10]
+    assert int(want.sum()) == 314
+    for adc, ntaps in {(a, t) for _, a, t, _ in rate_cases()}:
+        assert want[rate_rule.GRID == adc].all(), adc
+    for adc in (1_360_000, 1_520_000, 2_500_000, 5_800_000):
+        assert not rate_rule.well_defined(np.array([adc]))[0]
+    with pytest.raises(ValueError, match="past the end"):
+        Oracle(adc_rate=1_360_000)
+    with pytest.raises(ValueError):
+        Oracle(adc_rate=1_687_500)
