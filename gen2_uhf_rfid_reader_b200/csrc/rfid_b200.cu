@@ -310,17 +310,17 @@ int grow(rfid_b200_ctx* ctx, void** p, size_t* have, size_t need)
 }
 
 // Segments per CTA of rx_pack_kernel: as few CTAs as fill the device once (one CTA per SM, every SM busy for the
-// whole launch); larger batches run kPMaxSeg - 1 per CTA in several waves.  A CTA of kPMaxSeg segments lives about 1.4x
-// as long as one of kPMaxSeg - 1 (two of its decoder warps serve two segments, whose EPC windows are decoded one after
-// the other at the end, and its rings are shallower; H100 SXM, 400 W: 84-99 us against 63-77 us for cfg2's segments),
-// so it only pays where it saves a whole wave: batches of (kPMaxSeg - 1) * SMs + 1 .. kPMaxSeg * SMs segments.
+// whole launch); larger batches run kPMaxSeg per CTA in several waves.  With its decoder warps one pool over the
+// CTA's windows (rx_pack.cuh) a CTA of kPMaxSeg segments no longer decodes two EPC windows one after the other at its
+// end, and it does more work per SM than one of kPMaxSeg - 1 (H100 SXM, 700 W, two runs each: cfg3 6.20-6.21 ms
+// against 6.34-6.36 ms at kPMaxSeg - 1, cfg4 10.00-10.01 ms against 10.37-10.39 ms).
 int pack_segments_per_cta(const rfid_b200_ctx* ctx, int nseg)
 {
   if (ctx->pack_g_override > 0) return ctx->pack_g_override;
   const int sms = ctx->sm_count > 0 ? ctx->sm_count : 132;
   int g = (nseg + sms - 1) / sms;
   if (g < 1) g = 1;
-  if (g > kPMaxSeg) g = kPMaxSeg - 1;
+  if (g > kPMaxSeg) g = kPMaxSeg;
   return g;
 }
 

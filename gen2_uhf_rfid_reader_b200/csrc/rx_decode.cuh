@@ -208,6 +208,14 @@ struct WinStream {
   float2 h;
 };
 
+// lane t's candidate period of the symbol-period search, t_min + t (t_max - t_min) / 19 (:151-156; lanes 20..31 carry
+// t_min and are never read).  A caller that resumes a search from saved state recomputes it with this.
+__device__ __forceinline__ float win_stream_period(const RxConfig& c, int lane)
+{
+  const int number_steps = 20;
+  return f_add(c.t_min, f_div(f_mul((float)(lane < number_steps ? lane : 0), f_sub(c.t_max, c.t_min)), (float)(number_steps - 1)));
+}
+
 __device__ __forceinline__ int win_head_samples(const RxConfig& c, int kind, int n_total, int stage_cap)
 {
   return min(stage_cap, kind == RFID_B200_RN16 ? n_total : (int)(c.sync_range + 6.0f * c.n_tag_bit_f) + 2);
@@ -221,7 +229,9 @@ __device__ __forceinline__ int win_chunk_need(const RxConfig& c, const WinStream
   return min(n_total, lo + span);
 }
 
-// tag_sync + h_est; fills sync_index / score / h of `out` and the stream state
+// tag_sync + h_est; fills sync_index / score / h of `out` and the stream state.  progress = null: the whole window is
+// present, the head is loaded through L1.  A ProgressWait without a counter: the head's samples are present but the
+// window is still being written -- the head is loaded through L2 only, so that L1 keeps no line of the unwritten part.
 __device__ __forceinline__ void win_stream_head(const RxConfig& c, int kind, const WinSrc gw, int n_total,
                                                 float2* __restrict__ stage, int stage_cap, float2 dc, WinStream& S,
                                                 WindowDecode& out, ProgressWait* progress = nullptr)
@@ -277,8 +287,7 @@ __device__ __forceinline__ void win_stream_head(const RxConfig& c, int kind, con
   S.head = head;
   S.h = out.h;
   S.e = 0.0f;
-  const int number_steps = 20;
-  S.Tt = f_add(c.t_min, f_div(f_mul((float)(lane < number_steps ? lane : 0), f_sub(c.t_max, c.t_min)), (float)(number_steps - 1)));
+  S.Tt = win_stream_period(c, lane);
   S.phase = 1;
   asm volatile("" ::"f"(sink));
 }
@@ -310,6 +319,75 @@ __device__ __forceinline__ void win_stream_chunk(const RxConfig& c, const WinSrc
     S.e = e;
   }
   S.phase++;
+}
+
+// EPC, the symbol-period search complete: argmax, 128 bit decisions, CRC-16 (the end of win_stream_finish)
+__device__ __forceinline__ void win_stream_decide(const RxConfig& c, const WinSrc gw, int n_avail, float2* __restrict__ stage,
+                                                  int stage_cap, float2 dc, const WinStream& S, WindowDecode& out,
+                                                  ProgressWait* progress = nullptr, long long* pp = nullptr)
+{
+  const int lane = threadIdx.x & 31;
+  const int index = S.index;
+  const float2 h = S.h;
+  if (pp && lane == 0) pp[2] = clock64();
+  const int number_steps = 20;
+  const float min_val = c.t_min, max_val = c.t_max;
+  float energy = lane < number_steps ? S.e : -1.0f;
+  int e_idx = lane < number_steps ? lane : 0x7fffffff;
+  warp_argmax_first(energy, e_idx);
+  const int index_T = e_idx;
+  const float T = f_add(min_val, f_div(f_mul((float)index_T, f_sub(max_val, min_val)), (float)(number_steps - 1)));
+  out.T = T;
+  // ---- 128 bit decisions (:171-191), 32 pairs per stage fill
+  const float twoT = f_mul(2.0f, T);
+  unsigned Sg[4];
+  if (!progress) {
+    // the whole window is present: every lane gathers its eight samples straight from L2, all loads in flight together
+    float2 wa[4], wb[4];
+#pragma unroll
+    for (int r = 0; r < 4; r++) {
+      const int j = r * 32 + lane;
+      const int a = (int)f_add(f_mul((float)j, twoT), (float)index);
+      const int b = (int)f_add(f_add(f_mul((float)(j * 2), T), T), (float)index);
+      const bool ia = a >= 0 && a < n_avail, ib = b >= 0 && b < n_avail;   // (outside the window: 0, as the stage fill does)
+      wa[r] = ia ? __ldcg(gw.at(a)) : dc;
+      wb[r] = ib ? __ldcg(gw.at(b)) : dc;
+    }
+#pragma unroll
+    for (int r = 0; r < 4; r++) {
+      const int j = r * 32 + lane;
+      const int a = (int)f_add(f_mul((float)j, twoT), (float)index);
+      const int b = (int)f_add(f_add(f_mul((float)(j * 2), T), T), (float)index);
+      const float2 sa = (a >= 0 && a < n_avail) ? c_sub(wa[r], dc) : make_float2(0.f, 0.f);
+      const float2 sb = (b >= 0 && b < n_avail) ? c_sub(wb[r], dc) : make_float2(0.f, 0.f);
+      const float res = c_proj(sa, sb, h);
+      Sg[r] = __ballot_sync(0xffffffffu, res > 0.0f);
+    }
+  } else {
+#pragma unroll
+    for (int r = 0; r < 4; r++) {
+      const int j0 = r * 32;
+      const int lo = (int)f_add(f_mul((float)j0, twoT), (float)index);
+      stage_fill(stage, gw, lo, stage_cap, n_avail, progress, dc);
+      int j = j0 + lane;
+      int a = (int)f_add(f_mul((float)j, twoT), (float)index);
+      int b = (int)f_add(f_add(f_mul((float)(j * 2), T), T), (float)index);
+      float res = c_proj(stage[a - lo], stage[b - lo], h);
+      Sg[r] = __ballot_sync(0xffffffffu, res > 0.0f);
+    }
+  }
+  if (pp && lane == 0) pp[3] = clock64();
+  unsigned carry = 1u;
+#pragma unroll
+  for (int r = 0; r < 4; r++) {
+    unsigned prev = (Sg[r] << 1) | carry;
+    carry = Sg[r] >> 31;
+    unsigned Bv = Sg[r] ^ prev;
+    out.bits[r] = __brev(Bv);
+  }
+  out.crc_ok = crc16_check(out.bits);
+  out.tag_id = (int)((out.bits[3] >> 16) & 0xFFu);
+  if (pp && lane == 0) pp[4] = clock64();
 }
 
 // RN16: half-bit sampling + tag_detection_RN16 (:114-142, :237-253); EPC: remaining search chunks, argmax, 128 bit
@@ -434,65 +512,7 @@ __device__ __forceinline__ void win_stream_finish(const RxConfig& c, int kind, c
   } else {
     while (S.phase <= kSearchChunks) win_stream_chunk(c, gw, n_avail, stage, stage_cap, dc, S, progress);
   }
-  if (pp && lane == 0) pp[2] = clock64();
-  const int number_steps = 20;
-  const float min_val = c.t_min, max_val = c.t_max;
-  float energy = lane < number_steps ? S.e : -1.0f;
-  int e_idx = lane < number_steps ? lane : 0x7fffffff;
-  warp_argmax_first(energy, e_idx);
-  const int index_T = e_idx;
-  const float T = f_add(min_val, f_div(f_mul((float)index_T, f_sub(max_val, min_val)), (float)(number_steps - 1)));
-  out.T = T;
-  // ---- 128 bit decisions (:171-191), 32 pairs per stage fill
-  const float twoT = f_mul(2.0f, T);
-  unsigned Sg[4];
-  if (!progress) {
-    // the whole window is present: every lane gathers its eight samples straight from L2, all loads in flight together
-    float2 wa[4], wb[4];
-#pragma unroll
-    for (int r = 0; r < 4; r++) {
-      const int j = r * 32 + lane;
-      const int a = (int)f_add(f_mul((float)j, twoT), (float)index);
-      const int b = (int)f_add(f_add(f_mul((float)(j * 2), T), T), (float)index);
-      const bool ia = a >= 0 && a < n_avail, ib = b >= 0 && b < n_avail;   // (outside the window: 0, as the stage fill does)
-      wa[r] = ia ? __ldcg(gw.at(a)) : dc;
-      wb[r] = ib ? __ldcg(gw.at(b)) : dc;
-    }
-#pragma unroll
-    for (int r = 0; r < 4; r++) {
-      const int j = r * 32 + lane;
-      const int a = (int)f_add(f_mul((float)j, twoT), (float)index);
-      const int b = (int)f_add(f_add(f_mul((float)(j * 2), T), T), (float)index);
-      const float2 sa = (a >= 0 && a < n_avail) ? c_sub(wa[r], dc) : make_float2(0.f, 0.f);
-      const float2 sb = (b >= 0 && b < n_avail) ? c_sub(wb[r], dc) : make_float2(0.f, 0.f);
-      const float res = c_proj(sa, sb, h);
-      Sg[r] = __ballot_sync(0xffffffffu, res > 0.0f);
-    }
-  } else {
-#pragma unroll
-    for (int r = 0; r < 4; r++) {
-      const int j0 = r * 32;
-      const int lo = (int)f_add(f_mul((float)j0, twoT), (float)index);
-      stage_fill(stage, gw, lo, stage_cap, n_avail, progress, dc);
-      int j = j0 + lane;
-      int a = (int)f_add(f_mul((float)j, twoT), (float)index);
-      int b = (int)f_add(f_add(f_mul((float)(j * 2), T), T), (float)index);
-      float res = c_proj(stage[a - lo], stage[b - lo], h);
-      Sg[r] = __ballot_sync(0xffffffffu, res > 0.0f);
-    }
-  }
-  if (pp && lane == 0) pp[3] = clock64();
-  unsigned carry = 1u;
-#pragma unroll
-  for (int r = 0; r < 4; r++) {
-    unsigned prev = (Sg[r] << 1) | carry;
-    carry = Sg[r] >> 31;
-    unsigned Bv = Sg[r] ^ prev;
-    out.bits[r] = __brev(Bv);
-  }
-  out.crc_ok = crc16_check(out.bits);
-  out.tag_id = (int)((out.bits[3] >> 16) & 0xFFu);
-  if (pp && lane == 0) pp[4] = clock64();
+  win_stream_decide(c, gw, n_avail, stage, stage_cap, dc, S, out, progress, pp);
 }
 
 __device__ __forceinline__ void decode_window_staged(const RxConfig& c, int kind, const WinSrc gw, int n_avail,

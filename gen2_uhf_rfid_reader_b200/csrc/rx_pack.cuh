@@ -22,15 +22,19 @@
 //   warp B[g]   P3: thresholds by ballot (one mask word per lane), the edge / pulse state machine on the 256-bit masks, the
 //               DC-tracker inputs of the 48 samples after a window (y read back from the history), -0.0f for the samples
 //               inside windows.  Frees the |y| / quotient slot as soon as its masks are made.  Queues opening windows.
-//   warp C[d]   decodes the queued windows of segments g = d, d + D, ... straight from the history as soon as a window's
-//               last sample and its dc_est exist, whichever of its segments has one ready first (rx_decode.cuh); dc_est is
-//               subtracted as the decoder reads the samples -- the same exact float subtraction, gate_impl.cc:173,187.
-//               D = G while the CTA has room for 4G + 2 warps; at G = 8, D = 6 and warps C[0], C[1] serve two segments.
+//   warps C     D decoder warps, ONE pool over the queued windows of all G segments, straight from the history
+//               (rx_decode.cuh): any idle warp runs the next runnable phase of any segment's next window -- an EPC
+//               window's head and search chunks as soon as their samples and its dc_est exist, the rest once the whole
+//               window does; an RN16 window in one piece.  The state between phases is in shared memory (PackWinState).
+//               dc_est is subtracted as the decoder reads the samples -- the same exact float subtraction,
+//               gate_impl.cc:173,187.  D = G while the CTA has room for 4G + 2 warps, D = 6 at G = 8; warp A1[g] joins
+//               the pool once segment g is through P1, with the segment's raw stages as its decoder stage.
 //   loader      lane g streams segment g's raw samples through its two half-tile stages as warp A frees them.
 // The history is indexed by the SM (one CTA per SM: the shared-memory request guarantees it), so its size does not depend
 // on the number of segments of the launch; warp A never overwrites a sample a queued window still needs.
 // Shared memory per segment: 2 raw half-tile stages (10 KB), the last dc_length outputs of either half-tile (P1's DC
-// lookback is a lane shuffle plus this tail), a pas-tile ring of |y| (1 KB per tile); per decoder warp its stage (2 KB); per CTA
+// lookback is a lane shuffle plus this tail), a pas-tile ring of |y| (1 KB per tile), the decode state of its next
+// window (112 B, static); per decoder warp C its stage (2 KB; a warp A1 in the pool uses its segment's raw stages); per CTA
 // the running-sum buffers (pas + pds x 2 per segment, 1072 B each, skewed so the chain warp's 128-bit accesses are
 // bank-conflict free).  HBM traffic: every raw sample is read once (evict-first), 64 B are written per window; the history
 // (8 B per decimated sample, rewritten in place) lives in L2.
@@ -99,6 +103,19 @@ struct PackArgs {
   int smem_bytes;
 };
 
+// The decode of a segment's next window (sequence number n_decoded) between two of its phases (rx_decode.cuh: head,
+// search chunks, finish), which the decoder warps may run one after the other on different warps.  `ctl` = window
+// sequence number * 16 + next phase * 2 (+ 1 while a warp runs that phase); the candidate periods are recomputed
+// (win_stream_period), the energies e[] of candidates 0..19 are the only per-lane part.
+struct PackWinState {
+  volatile int ctl;
+  int index, head, sync_index;
+  float score;
+  float2 h;
+  float e[20];
+};
+__device__ __forceinline__ int pws_ctl(int k, int phase) { return k * 16 + phase * 2; }
+
 struct PackSegCtl {
   rfid_b200_segment seg;     // the segment's table entry (length 0: none), read from global memory once per CTA
   uint64_t raw_full[2];      // loader (TMA transaction count) -> warp A
@@ -117,6 +134,7 @@ struct PackSegCtl {
   int n_e[kPDSMax];           // closed samples of the tile in DC-list slot (written by P3)
   int trig_n[kPDSMax];        // queued windows that opened in that tile: index of the trigger in the list, sequence number
   int trig_j[kPDSMax][kPTrig], trig_k[kPDSMax][kPTrig];
+  PackWinState w;            // the decode of window n_decoded (warps C)
 };
 struct PackCtaCtl {
   uint64_t fullA[kPASMax];    // 2G warps A -> chain: P1 of the tile is in
@@ -251,6 +269,54 @@ __device__ __forceinline__ int fsm_closed_run_lanes(unsigned ltw, unsigned gtw, 
   return -1;
 }
 
+// One claimed phase of a window's decode (decoder pool): act 1 the head, 2 one chunk of the symbol-period search, 3 the
+// rest (the head if not yet run, the remaining chunks, bit decisions, CRC) and the record.  The decode's state comes
+// from and goes back to W (rx_decode.cuh's WinStream / WindowDecode: the arithmetic of decode_window_staged, resumed).
+__device__ __forceinline__ void pack_decode_phase(const RxConfig& C, PackWinState& W, int kind, const WinSrc wv, int len,
+                                               float2* dstage, int stage_cap, float2 dc, int phase, int act,
+                                               rfid_b200_window_result* dst, int seg_id, int ord, int wopen, float2* tap,
+                                               long long* pe)
+{
+  const int lane = threadIdx.x & 31;
+  WinStream S;
+  WindowDecode wd;
+  if (phase == 0) {
+    // the whole window present: the head through L1, as decode_window_staged; else through L2 only
+    ProgressWait l2_only{nullptr, nullptr, 0u};
+    win_stream_head(C, kind, wv, len, dstage, stage_cap, dc, S, wd, act == 3 ? nullptr : &l2_only);
+    if (pe && lane == 0) pe[1] = clock64();
+  } else {
+    S.phase = phase; S.index = W.index; S.head = W.head; S.h = W.h;
+    S.e = lane < 20 ? W.e[lane] : 0.0f;
+    S.Tt = win_stream_period(C, lane);
+    wd.sync_index = W.sync_index; wd.score = W.score; wd.h = W.h;
+    wd.bits[0] = wd.bits[1] = wd.bits[2] = wd.bits[3] = 0u;
+  }
+  if (act == 2) {
+    const long long t = pe ? clock64() : 0;
+    win_stream_chunk(C, wv, len, dstage, stage_cap, dc, S);
+    if (pe && lane == 0) { pe[5] += clock64() - t; pe[7]++; }
+  }
+  if (act == 3) {
+    if (pe && lane == 0) pe[6] = clock64();
+    if (kind == RFID_B200_RN16) {
+      win_stream_finish(C, kind, wv, len, dstage, stage_cap, dc, S, wd, nullptr, pe);
+    } else {
+      // chunk by chunk, not win_stream_finish's search: that one keeps the next chunk's samples in 24 registers while a
+      // chunk runs, which in this kernel (64 registers per thread) leaves ptxas none for the chunk's gathers -- every
+      // step became one dependent chain of index, gather and add.  Here a chunk's eight gathers are in flight together.
+      while (S.phase <= kSearchChunks) win_stream_chunk(C, wv, len, dstage, stage_cap, dc, S);
+      win_stream_decide(C, wv, len, dstage, stage_cap, dc, S, wd, nullptr, pe);
+    }
+    if (lane == 0) store_result(dst, wd, seg_id, ord, wopen, len, kind);
+    if (tap)
+      for (int p2 = lane; p2 < len; p2 += 32) tap[p2] = c_sub(__ldcg(wv.at(p2)), dc);
+  } else {
+    if (lane < 20) W.e[lane] = S.e;
+    if (lane == 0) { W.index = S.index; W.head = S.head; W.h = S.h; W.sync_index = wd.sync_index; W.score = wd.score; }
+  }
+}
+
 // PAS = pack_ring_slots(G) of the launch (PackArgs::pas): the ring indices stay compile-time divisions
 template <int DECIM, int MFQ, int PAS>
 __global__ void __launch_bounds__(kPackMaxThreads, 1) rx_pack_kernel(const PackArgs A)
@@ -262,8 +328,8 @@ __global__ void __launch_bounds__(kPackMaxThreads, 1) rx_pack_kernel(const PackA
   __shared__ long long pp_cta_t0;
   if (threadIdx.x == 0) pp_cta_t0 = clock64();
   int pp_step = 0;
-  // per-CTA start / end on the global timer (ns): rows 512.. of the log
-  unsigned long long* pp_cta = A.window_tap ? reinterpret_cast<unsigned long long*>(A.window_tap) + 512 * 8 + 2 * blockIdx.x : nullptr;
+  // per CTA on the global timer (ns), rows 512.. of the log: start, last decode done, last window closed by a gate
+  unsigned long long* pp_cta = A.window_tap ? reinterpret_cast<unsigned long long*>(A.window_tap) + 512 * 8 + 4 * blockIdx.x : nullptr;
   if (pp_cta && threadIdx.x == 0) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); pp_cta[0] = t; }
 #endif
 
@@ -310,6 +376,7 @@ __global__ void __launch_bounds__(kPackMaxThreads, 1) rx_pack_kernel(const PackA
       for (int s = 0; s < PDS; s++) { c.n_e[s] = 0; c.trig_n[s] = 0; }
       c.n_opened = 0; c.n_dc = 0; c.n_decoded = 0; c.seg_done = 0; c.y_tiles = 0;
       c.b_wcount = 0; c.b_nq = 1; c.b_snap_base = 0; c.b_queued = 0;
+      c.w.ctl = pws_ctl(0, 0);
       mbar_fence_init();
     }
     if (threadIdx.x == 32) {
@@ -334,6 +401,9 @@ __global__ void __launch_bounds__(kPackMaxThreads, 1) rx_pack_kernel(const PackA
     }
   }
 
+  // the decoder pool (below): warps C from the start, each with its stage; warp A1[g] once segment g is through P1
+  float2* pool_stage = nullptr;
+  int pool_id = 0;
   if (warp < 3 * G) {
     // ======================================================================================= warps A0 / A1 (P1) and B (P3)
     const bool is_a = warp < 2 * G;
@@ -751,6 +821,9 @@ __global__ void __launch_bounds__(kPackMaxThreads, 1) rx_pack_kernel(const PackA
                 n_e = pos;
                 if (n_samples >= to_ungate) {
                   gate_open = false;
+#ifdef RFID_B200_PHASE_PROFILE
+                  if (pp_cta && lane == 0) { unsigned long long tg; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(tg)); atomicMax(pp_cta + 2, tg); }
+#endif
                   const int wcount = B.b_wcount, nq = B.b_nq;
                   const int kind = wcount & 1;  // windows alternate RN16, EPC (SURVEY.md 3.5)
                   __syncwarp();
@@ -903,88 +976,138 @@ __global__ void __launch_bounds__(kPackMaxThreads, 1) rx_pack_kernel(const PackA
       issue(k);
     }
   } else {
-    // ======================================================================================= warps C: decode
-    // warp d serves segments d, d + D, ...: the windows of a segment in order (n_decoded, warp A's guard of the history,
-    // keeps its meaning), and of its segments whichever has its next window decodable first -- it never waits on one
-    // segment while another one has a window ready.  A window is decodable as soon as its last sample is in the history
-    // (warp A runs ahead of the gate) and dc_est right after its trigger sample has come from the chain warp (two tiles
-    // after the gate opened it).
-    const int D = pack_decoders(G);
-    const int d = warp - 3 * G - 2;
-    PP_DECL
+    pool_stage = reinterpret_cast<float2*>(smem + A.off_dstage) + (size_t)(warp - 3 * G - 2) * A.dstage_samples;
+    pool_id = warp - 3 * G - 2;
+  }
+  if (warp >= G && warp < 2 * G) {
+    // Warp A1[g] once segment g is through P1 (recomputed here: nothing of the pool stays live through P1's loop).  The
+    // segment's raw stages are free once its last tile is in the history (y_tiles moves after the tile's last read of
+    // them; a lone first half is warp A0's, and the loader's last copy went to it): warp A1 joins the decoder pool with
+    // them as its stage -- the segments' last windows close towards the end of the CTA, when warps A are done.
+    const int g = warp - G;
+    if (g < g_act) {
+      const int ntiles = ((int)(ctl_all[g].seg.length / DECIM) + kT2 - 1) / kT2;
+      while (ctl_all[g].y_tiles < ntiles) __nanosleep(200);
+    }
+    pool_stage = reinterpret_cast<float2*>(smem + A.off_seg + (size_t)g * A.seg_bytes + A.o_raw);
+    pool_id = pack_decoders(G) + g;
+  }
+  if (pool_stage) {
+    // ======================================================================================= decoder pool: warps C, A1
+    // The decoder warps are ONE pool over the phases of every segment's next window (rx_decode.cuh): the head of an EPC
+    // window and the chunks of its symbol-period search may run as soon as the samples they read are in the history,
+    // while the gate is still receiving the window (warp A runs ahead of it), and its finish (the remaining chunks, the
+    // 128 bit decisions, the CRC) once the whole window is; an RN16 window is one unit (its finish reads the stage its
+    // head filled).  Every phase needs dc_est right after the window's trigger sample, which the chain warp hands over
+    // two tiles after the gate opened the window -- by then warp A is about a tile short of the window's end, so the head
+    // usually runs early and the chunks rarely (tools/pack_profile.py).  An idle warp takes the runnable phase of the
+    // window with the most phases left (lowest segment first among equals) and claims it by a compare-and-swap on the
+    // window's ctl word: one phase of a window runs at a time, and its state between phases lives in PackSegCtl::w.  A
+    // segment's windows finish in order and n_decoded moves only after the finish, so warp A's guard of the history
+    // keeps its meaning.  Which warp runs a phase does not change its result: the records are the same bits.
+    float2* const dstage = pool_stage;
+    const unsigned FULL = 0xffffffffu;
 #ifdef RFID_B200_PHASE_PROFILE
-    long long* const pp_c0 = (seg0 == 0 && d == 0 && A.window_tap) ? reinterpret_cast<long long*>(A.window_tap) + 192 * 8 : nullptr;
-    int pp_seen = 0;   // windows of segment 0 whose opening has been stamped
+    // segment 0 of CTA 0: per window k, row k = opened seen, first phase starts, decoded, finish starts (cycles since
+    // CTA start); rows 60 (EPC) / 61 (RN16): clock64() at head start, head end, search end, bit samples end, CRC end,
+    // cycles spent in search chunks before the finish, finish start, number of those chunks
+    long long* const pp_c0 = (seg0 == 0 && A.window_tap) ? reinterpret_cast<long long*>(A.window_tap) + 192 * 8 : nullptr;
 #endif
     while (true) {
-      // lane 0 looks, the warp follows (every lane must decode the same window): the segment to serve, or -1 nothing
-      // opened, -2 a window opened but not decodable yet, -3 every segment of this warp over
-      int pick = -3, k = 0;
-      if (lane == 0) {
-        for (int g = d; g < g_act; g += D) {
-          PackSegCtl& S = ctl_all[g];
-          const int done = S.seg_done;   // (read before the counters: once set, they are final)
-          const int kg = S.n_decoded, no = S.n_opened;
-          if (no <= kg) {
-            if (!done && pick == -3) pick = -1;
-            continue;
-          }
+      // lane g looks at segment g: is its next window's next phase runnable (key > 0), is anything left (pending)
+      bool pending = false;
+      unsigned key = 0u;       // (phases left + 1) * 16 + 15 - g
+      int st = 0, act = 0;     // the ctl word seen; what to run: 1 the head, 2 one search chunk, 3 the rest of the decode
+      if (lane < g_act) {
+        PackSegCtl& S = ctl_all[lane];
+        const int done = S.seg_done;   // (read before the counters: once set, they are final)
+        const int kg = S.n_decoded, no = S.n_opened;
+        pending = no > kg || !done;
+        if (no > kg) {
           __threadfence_block();
 #ifdef RFID_B200_PHASE_PROFILE
-          if (pp_c0 && g == 0 && kg >= pp_seen) { pp_c0[kg * 8] = clock64() - pp_cta_t0; pp_seen = kg + 1; }
+          if (pp_c0 && lane == 0 && pp_c0[kg * 8] == 0) pp_c0[kg * 8] = clock64() - pp_cta_t0;
 #endif
-          const int qs0 = kg & (kPQ - 1);
-          const int wend = S.q_open[qs0] + (S.q_kind[qs0] ? C.len_epc : C.len_rn16);
-          if (S.y_tiles * kT2 >= wend && S.n_dc > kg) { pick = g; k = kg; break; }
-          pick = -2;
+          st = S.w.ctl;
+          if ((st >> 4) == kg && !(st & 1) && S.n_dc > kg) {
+            const int qs = kg & (kPQ - 1);
+            const int kind = S.q_kind[qs];
+            const int len = kind ? C.len_epc : C.len_rn16;
+            const int avail = S.y_tiles * kT2 - S.q_open[qs];   // the window's samples in the history
+            const int phase = (st >> 1) & 7;
+            if (avail >= len) {
+              act = 3;
+            } else if (kind && phase == 0) {
+              act = avail >= win_head_samples(C, kind, len, A.dstage_samples) ? 1 : 0;
+            } else if (kind && phase <= kSearchChunks) {
+              WinStream ws;
+              ws.index = S.w.index;
+              act = avail >= win_chunk_need(C, ws, phase - 1, len, A.dstage_samples) ? 2 : 0;
+            }
+            if (act) key = (unsigned)(kind ? kSearchChunks + 3 - phase : 2) * 16u + 15u - (unsigned)lane;
+          }
         }
       }
-      pick = __shfl_sync(0xffffffffu, pick, 0);
-      if (pick == -3) break;
-      if (pick < 0) {
-        __nanosleep(pick == -1 ? 400 : 200);   // (-1: nothing to do until warp B opens a window)
-        continue;
-      }
-      k = __shfl_sync(0xffffffffu, k, 0);
-      const int g = pick;
+      if (!__any_sync(FULL, pending)) break;
+      const unsigned best = __reduce_max_sync(FULL, key);
+      if (best == 0u) { __nanosleep(200); continue; }
+      const int g = 15 - (int)(best & 15u);
+      int won = 0;
+      if (lane == g) won = atomicCAS(const_cast<int*>(&ctl_all[g].w.ctl), st, st | 1) == st;
+      if (!__shfl_sync(FULL, won, g)) continue;   // another warp was first
+      st = __shfl_sync(FULL, st, g);
+      act = __shfl_sync(FULL, act, g);
+      __threadfence_block();
+      const int k = st >> 4, phase = (st >> 1) & 7;
       const int seg = seg0 + g;
       PackSegCtl& B = ctl_all[g];
-      const float2* const y_seg = y_cta + (size_t)g * kYW;
-      float2* const dstage = reinterpret_cast<float2*>(smem + A.off_dstage) + (size_t)d * A.dstage_samples;   // this warp's
+      PackWinState& W = B.w;
+      const int qs = k & (kPQ - 1);
+      const int kind = B.q_kind[qs], ord = B.q_ord[qs], wopen = B.q_open[qs];
+      const float2 dc = B.dc_val[qs];
+      const int len = kind ? C.len_epc : C.len_rn16;
+      const WinSrc wv{y_cta + (size_t)g * kYW, wopen, kYW - 1};
 #ifdef RFID_B200_PHASE_PROFILE
-      pp_log = seg == 0 ? pp_c0 : nullptr;
-      pp_step = k;
-#endif
-      {
-        __threadfence_block();
-        const int qs = k & (kPQ - 1);
-        const int kind = B.q_kind[qs], ord = B.q_ord[qs], wopen = B.q_open[qs];
-        const float2 dc = B.dc_val[qs];
-        const int len = kind ? C.len_epc : C.len_rn16;
-        const WinSrc wv{y_seg, wopen, kYW - 1};
-        PP_AT(1)
-        WindowDecode wd;
-#ifdef RFID_B200_PHASE_PROFILE
-        decode_window_staged(C, kind, wv, len, dstage, A.dstage_samples, wd, nullptr, nullptr, dc, pp_log ? pp_log + (kind ? 60 : 61) * 8 : nullptr);
-#else
-        decode_window_staged(C, kind, wv, len, dstage, A.dstage_samples, wd, nullptr, nullptr, dc);
-#endif
-        rfid_b200_window_result* dst = A.results + (size_t)seg * A.max_windows + ord;
-        if (lane == 0) store_result(dst, wd, seg + A.seg_base, ord, wopen, len, kind);
-#ifndef RFID_B200_PHASE_PROFILE
-        if (A.window_tap) {
-          float2* tap = A.window_tap + ((size_t)(seg + A.seg_base) * A.max_windows + ord) * C.len_epc;
-          for (int p2 = lane; p2 < len; p2 += 32) tap[p2] = c_sub(__ldcg(wv.at(p2)), dc);
-        }
-#endif
-        __syncwarp();
-        if (lane == 0) { __threadfence_block(); B.n_decoded = k + 1; }   // warp A may reuse the window's history samples
-        PP_AT(2)
+      long long* const pw = (pp_c0 && g == 0) ? pp_c0 : nullptr;
+      long long* const pe = pw ? pw + (kind ? 60 : 61) * 8 : nullptr;
+      const long long pp_t = clock64();
+      // every claim of CTA 0 (rows 1024..; count at row 1023): warp | segment | window | what | phase, start, end
+      long long* pp_claim = nullptr;
+      if (pp_c0 && lane == 0) {
+        const long long n = atomicAdd(reinterpret_cast<unsigned long long*>(pp_c0) + (1023 - 192) * 8, 1ull);
+        if (n < 1024) pp_claim = pp_c0 + (1024 - 192) * 8 + 4 * n;
       }
-    }
-#ifdef RFID_B200_PHASE_PROFILE
-    if (pp_cta && d < g_act && lane == 0) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); atomicMax(pp_cta + 1, t); }
+      if (pp_claim) { pp_claim[0] = pool_id | g << 8 | k << 16 | act << 24 | phase << 28; pp_claim[1] = pp_t - pp_cta_t0; }
+      if (pw && lane == 0 && phase == 0) { pw[k * 8 + 1] = pp_t - pp_cta_t0; pe[0] = pp_t; pe[5] = 0; pe[7] = 0; }
+      if (pw && lane == 0 && act == 3) pw[k * 8 + 3] = pp_t - pp_cta_t0;
+      float2* const tap = nullptr;   // (the profile log)
+#else
+      long long* const pe = nullptr;
+      float2* const tap = A.window_tap ? A.window_tap + ((size_t)(seg + A.seg_base) * A.max_windows + ord) * C.len_epc : nullptr;
 #endif
+      pack_decode_phase(C, W, kind, wv, len, dstage, A.dstage_samples, dc, phase, act,
+                        A.results + (size_t)seg * A.max_windows + ord, seg + A.seg_base, ord, wopen, tap, pe);
+      __syncwarp();
+      if (act == 3) {
+#ifdef RFID_B200_PHASE_PROFILE
+        if (pw && lane == 0) pw[k * 8 + 2] = clock64() - pp_cta_t0;
+        if (pp_cta && lane == 0) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); atomicMax(pp_cta + 1, t); }
+#endif
+        if (lane == 0) {
+          // the next window's state first: a warp that still reads n_decoded == k sees a ctl word of window k + 1
+          __threadfence_block();
+          W.ctl = pws_ctl(k + 1, 0);
+          __threadfence_block();
+          B.n_decoded = k + 1;   // warp A may reuse the window's history samples
+        }
+      } else if (lane == 0) {
+        __threadfence_block();
+        W.ctl = pws_ctl(k, act == 1 ? 1 : phase + 1);
+      }
+#ifdef RFID_B200_PHASE_PROFILE
+      if (pp_claim) pp_claim[2] = clock64() - pp_cta_t0;
+#endif
+    }
   }
 }
 

@@ -1,6 +1,7 @@
 #!/usr/bin/env python
 """Developer aid: build the library with RFID_B200_PHASE_PROFILE and print the timeline (cycles since CTA start) of the
-pack kernel's warps A / B / C of segment 0 and of the chain warp of CTA 0 (GPU box).  RFID_B200_LIB selects an already
+pack kernel's warps A / B / C of segment 0 and of the chain warp of CTA 0, the decode phases of segment 0's windows, and
+per CTA its lifetime and the time from its last window closing at a gate to its last decode done (GPU box).  RFID_B200_LIB selects an already
 built profiling library instead; RFID_B200_PACK_G forces the segments per CTA (as in the library)."""
 import os, sys, subprocess
 import numpy as np, torch
@@ -33,11 +34,14 @@ sms = torch.cuda.get_device_properties(dev).multi_processor_count
 G = int(os.environ.get("RFID_B200_PACK_G", "0")) or min(PACK_MAX_SEG, max(1, -(-nseg // sms)))
 ncta = (nseg + G - 1) // G
 print("G = %d segments per CTA, %d CTAs on %d SMs" % (G, ncta, sms))
-ct = raw_log[512 * 8: 512 * 8 + 2 * ncta].reshape(ncta, 2).astype(np.float64)
+ct = raw_log[512 * 8: 512 * 8 + 4 * ncta].reshape(ncta, 4)[:, :3].astype(np.float64)
 t0 = ct[:, 0].min()
-st, en = (ct[:, 0] - t0) / 1000.0, (ct[:, 1] - t0) / 1000.0
-print("CTAs %d: start us min %.2f max %.2f | last decode done us: min %.2f p50 %.2f p90 %.2f max %.2f | CTA 0: %.2f .. %.2f" %
-      (ncta, st.min(), st.max(), en.min(), np.percentile(en, 50), np.percentile(en, 90), en.max(), st[0], en[0]))
+st, en, cl = (ct[:, 0] - t0) / 1000.0, (ct[:, 1] - t0) / 1000.0, (ct[:, 2] - t0) / 1000.0
+life, tail = en - st, en - cl
+pct = lambda v: "min %.2f p50 %.2f p90 %.2f max %.2f" % (v.min(), np.percentile(v, 50), np.percentile(v, 90), v.max())
+print("CTAs %d: start us min %.2f max %.2f | last decode done us: %s | CTA 0: %.2f .. %.2f" % (ncta, st.min(), st.max(), pct(en), st[0], en[0]))
+print("CTA lifetime us: %s" % pct(life))
+print("last window closed by a gate -> last decode done, us: %s" % pct(tail))
 order = np.argsort(en)
 print("slowest CTAs:", [(int(i), round(float(en[i]), 2)) for i in order[-6:]], "fastest:", [(int(i), round(float(en[i]), 2)) for i in order[:4]])
 A, B, CH, C = log[0:64], log[64:128], log[128:192], log[192:256]
@@ -51,7 +55,19 @@ for i in range(steps):
     print("%3d | %7d %7d %7d %7d | %7d %7d | %7d %7d %7d | %7d %7d %7d" %
           (i, A[i][0], A[i][1], A[i][2], A[i][3], A1[i][0], A1[i][3], B[i][0], B[i][1], B[i][2], CH[i][0], CH[i][1], CH[i][2]))
 for k in range(2):
-    print("window %d: close seen %d, dc ready %d, decoded %d" % (k, C[k][0], C[k][1], C[k][2]))
-for name, d in (("EPC", C[60]), ("RN16", C[61])):
-    print("%s decode of segment 0 (cycles): head+sync %d, period search %d, bit samples %d, bits+crc %d, total %d" %
-          (name, d[1] - d[0], d[2] - d[1], d[3] - d[2], d[4] - d[3], d[4] - d[0]))
+    print("window %d: opened seen %d, first phase %d, finish starts %d, decoded %d" % (k, C[k][0], C[k][1], C[k][3], C[k][2]))
+e = C[60]
+print("EPC decode of segment 0 (cycles of work): head+sync %d, period search %d in %d chunks before the finish + %d in it, "
+      "bit samples %d, bits+crc %d; finish %d" % (e[1] - e[0], e[5], e[7], e[2] - e[6], e[3] - e[2], e[4] - e[3], e[4] - e[6]))
+r = C[61]
+print("RN16 decode of segment 0 (cycles): head+sync %d, bit decisions %d, total %d" % (r[1] - r[0], r[4] - r[6], r[4] - r[0]))
+nclaim = int(raw_log[1023 * 8])
+if nclaim:
+    cl = raw_log[1024 * 8: 1024 * 8 + 4 * min(nclaim, 1024)].reshape(-1, 4)
+    what = {1: "head", 2: "chunk", 3: "rest"}
+    print("decoder claims of CTA 0 (%d), by pool warp (C0.., then A1 of segment id - D): segment/window what@phase start-end" % nclaim)
+    for d in sorted(set(int(c[0]) & 0xff for c in cl)):
+        rows = sorted((c for c in cl if int(c[0]) & 0xff == d), key=lambda c: c[1])
+        busy = sum(int(c[2] - c[1]) for c in rows)
+        print("  C%d busy %d:" % (d, busy), " ".join("%d/%d %s@%d %d-%d" % ((int(c[0]) >> 8) & 0xff, (int(c[0]) >> 16) & 0xff,
+              what.get((int(c[0]) >> 24) & 0xf, "?"), (int(c[0]) >> 28) & 0xf, c[1], c[2]) for c in rows))
