@@ -176,16 +176,16 @@ int align_up(int v, int a) { return (v + a - 1) / a * a; }
 
 bool fast_path_ok(const RxConfig& c) { return c.win_length <= kTT && c.dc_length <= kTT; }
 
-// smallest decoder stage for a window that is complete when the decode starts: the head (sync range + 6 symbols) and one
-// chunk of the symbol-period search (one float per sample); the bit decisions and the rest of an RN16 window are read from
-// global memory directly
-int decode_stage_small(const RxConfig& c)
+// Decoder stage (float2 samples) of one decoder warp of the pack, split and block-mode kernels (rx_decode.cuh, STAGED):
+// the window's head (sync range + 6 symbols), one chunk of the symbol-period search (win_chunk_span samples at one float
+// each) and an RN16 window whole.  The bit decisions read global memory directly.
+int head_stage_samples(const RxConfig& c) { return align_up(c.sync_range + (int)(6.0f * c.n_tag_bit_f) + 2, 8); }
+int chunk_stage_samples(const RxConfig& c)
 {
-  const int head = c.sync_range + (int)(6.0f * c.n_tag_bit_f) + 2;
-  const int span = (int)((float)kChunkSteps * c.t_max + 256.0f * (c.t_max - c.t_min)) + 8;
-  int need = head > (span + 1) / 2 ? head : (span + 1) / 2;
-  return align_up(need, 8);
+  return align_up(std::max({head_stage_samples(c), (win_chunk_span(c) + 1) / 2, c.len_rn16}), 8);
 }
+// rx_fused_kernel stages the head only (head_stage_samples): its long rings leave little shared memory, so its search
+// chunks and the rest of its RN16 windows gather from L2.
 
 // shared-memory carve-up of rx_fused_split_kernel: five tile stages forming one time-indexed ring
 void make_layout_split(const RxConfig& c, FusedArgs& L)
@@ -200,8 +200,7 @@ void make_layout_split(const RxConfig& c, FusedArgs& L)
   L.off_tile_d = off; off += kRing * 4 + 64;          // + read-ahead pad of the running-sum loop
   L.off_etile = off; off += kS * 2 * kTT * 4 + 64;
   L.off_snap = off; off = align_up(off + c.dc_length * 8, 16);
-  L.dstage_samples = decode_stage_samples(c.n_tag_bit_f);
-  if (L.dstage_samples < c.len_rn16) L.dstage_samples = align_up(c.len_rn16, 8);  // an RN16 window is staged whole
+  L.dstage_samples = chunk_stage_samples(c);
   L.off_dstage = off; off = align_up(off + L.dstage_samples * 8, 16);
   L.ahist_size = L.ycl_size = 0;
   L.off_ahist = L.off_ycl = L.off_e = 0;
@@ -234,8 +233,7 @@ void make_layout(const RxConfig& c, FusedArgs& L)
     L.off_ycl = off; off = align_up(off + L.ycl_size * 8, 16);
     L.off_e = off; off += 2 * (kTT + 16) * 4;
   }
-  // (long rings leave little shared memory: the decoder stages the window's head only and gathers the rest from L2)
-  L.dstage_samples = align_up(c.sync_range + (int)(6.0f * c.n_tag_bit_f) + 2, 8);
+  L.dstage_samples = head_stage_samples(c);
   L.off_dstage = off; off = align_up(off + L.dstage_samples * 8, 16);
   L.rn16_pad = align_up(c.len_rn16, 16);
   L.win_stride = L.rn16_pad + align_up(c.len_epc, 16);
@@ -271,10 +269,7 @@ void make_layout_pack(const RxConfig& c, int G, PackArgs& L)
   L.o_tail_y = o; o = align_up(o + 2 * c.dc_length * 8, 16);
   L.o_ring_a = o; o += L.pas * kT2 * 4;
   L.seg_bytes = align_up(o, 16);
-  // decode stage, one per decoder warp: an RN16 window is staged whole; an EPC window needs its head and one chunk of the
-  // period search
-  L.dstage_samples = decode_stage_small(c);
-  if (L.dstage_samples < c.len_rn16) L.dstage_samples = align_up(c.len_rn16, 8);
+  L.dstage_samples = chunk_stage_samples(c);   // one per decoder warp
   int off = 0;
   L.off_dA = off; off += L.pas * G * kPChainBuf * 4;
   L.off_dD = off; off += L.pds * 2 * G * kPChainBuf * 4;
@@ -456,7 +451,7 @@ int rfid_b200_create(const rfid_b200_params* p, rfid_b200_ctx** out)
     e = cudaFuncSetAttribute((const void*)fn, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   if (e == cudaSuccess)
     e = cudaFuncSetAttribute((const void*)decode_block_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             cfg.len_epc * 12 + 64);
+                             chunk_stage_samples(cfg) * 8);
   if (e != cudaSuccess) {
     cudaGetLastError();
     rfid_b200_destroy(ctx);
@@ -1222,7 +1217,8 @@ int rfid_b200_decoder_work(rfid_b200_ctx* ctx, int kind, const float* win, int n
   if ((rc = grow(ctx, &ctx->d_in, &ctx->d_in_bytes, (size_t)need * 8))) return rc;
   cudaStream_t s = ctx->stream;
   CK(cudaMemcpyAsync(ctx->d_in, win, (size_t)need * 8, cudaMemcpyHostToDevice, s));
-  decode_block_kernel<<<1, 32, (size_t)need * 12 + 64, s>>>(ctx->cfg, kind, (const float2*)ctx->d_in, need, ctx->d_one);
+  const int stage = chunk_stage_samples(ctx->cfg);
+  decode_block_kernel<<<1, 32, (size_t)stage * 8, s>>>(ctx->cfg, kind, (const float2*)ctx->d_in, need, stage, ctx->d_one);
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(res, ctx->d_one, sizeof(*res), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));

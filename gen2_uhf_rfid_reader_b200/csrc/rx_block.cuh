@@ -122,11 +122,11 @@ __global__ void __launch_bounds__(32) gate_block_kernel(RxConfig C, GateState* s
 
 // tag_decoder_impl::general_work on one window (tag_decoder_impl.cc:223-393)
 __global__ void __launch_bounds__(32) decode_block_kernel(RxConfig C, int kind, const float2* __restrict__ win_g, int n,
-                                                          rfid_b200_window_result* res)
+                                                          int stage_cap, rfid_b200_window_result* res)
 {
-  extern __shared__ __align__(16) unsigned char dsm[];   // 12 n + 64 bytes: a decoder stage of 1.5 n samples
+  extern __shared__ __align__(16) float2 dstage[];   // the decoder stage: stage_cap samples
   WindowDecode wd;
-  decode_window_staged(C, kind, win_g, n, reinterpret_cast<float2*>(dsm), n + n / 2, wd);
+  decode_window_staged<true>(C, kind, win_g, n, dstage, stage_cap, wd);
   if (threadIdx.x == 0)
     store_result(res, wd, 0, 0, 0, kind == RFID_B200_RN16 ? C.len_rn16 : C.len_epc, kind);
 }

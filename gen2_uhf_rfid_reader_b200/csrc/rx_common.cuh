@@ -221,17 +221,6 @@ __device__ __forceinline__ void mbar_wait_idle(uint64_t* bar, uint32_t parity, u
 {
   while (!mbar_try_wait(bar, parity)) __nanosleep(sleep_ns);
 }
-// one try_wait with a suspend-time hint: true when the phase of parity `parity` has completed; false after (about) hint_ns
-__device__ __forceinline__ bool mbar_try_wait_hint(uint64_t* bar, uint32_t parity, uint32_t hint_ns)
-{
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity), "r"(hint_ns)
-      : "memory");
-  return ok != 0;
-}
 // 1-D bulk copy global -> shared through the TMA engine; completion is signalled on `bar`
 // (SASS: UBLKCP).  dst/src 16-byte aligned, bytes a multiple of 16.
 __device__ __forceinline__ void tma_load_1d(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar)

@@ -50,42 +50,29 @@ __device__ __forceinline__ int crc16_check(const uint32_t bits[4])
 // ---------------------------------------------------------------------------------------------------------
 // The decoder of one window (tag_decoder_impl.cc:78-191, 223-393), ONE copy for every kernel: the window lives in global
 // memory (a capture kernel's L2-resident scratch / history, or the block-mode input buffer); the warp copies the part of
-// the window it is about to use into a small shared-memory stage with coalesced loads and gathers from there.
+// the window it is about to gather from many times into a small shared-memory stage with coalesced loads and gathers from
+// there; the 256 samples of the bit decisions are gathered from L2 directly.
 // w = y - dc_est: dc is subtracted as the samples are loaded (one exact float subtraction, gate_impl.cc:173,187).
 // All 32 lanes of the warp must call; the result is valid in every lane.  The stage must hold the window head (sync range +
-// 6 symbols); with room for a chunk of the symbol-period search the search runs from the stage, else it gathers from L2.
-__host__ __device__ inline int decode_stage_samples(float n_tag_bit)
-{
-  // one chunk = 32 consecutive bit pairs: 31 symbols + one half symbol at the longest candidate period, + slack
-  return ((int)(32.5f * n_tag_bit * 1.0101f) + 16 + 7) & ~7;
-}
+// 6 symbols); with room for a chunk of the symbol-period search the search runs from the stage, else it gathers from L2
+// (win_stream_chunk).
 
-// `progress` (may be null): number of window samples the producer has published so far; the fill waits until
-// the range it is about to read exists.  This is what lets the decoder work on a window WHILE it is still being
-// gated (streaming decode), instead of starting when the window closes.
-#ifndef RFID_B200_PROGRESS_NS
-#define RFID_B200_PROGRESS_NS 300
-#endif
-// How the decoder waits for window samples that are still being gated: `counter` = samples published so far.  With a
-// doorbell (an mbarrier the producer arrives on after every publication) the waiting warp is parked by the hardware;
-// without one it polls the counter with a sleep in between.  The counter, not the doorbell's phase, decides: every wait
-// is bounded (suspend hint), so a phase that was rung before the warp looked only costs one time-out.
+// `progress` (may be null): how the decoder waits for window samples that are still being gated.  `counter` = number of
+// window samples the producer has published so far; a reader polls it, with a sleep in between, until the range it is
+// about to read exists.  This is what lets the decoder work on a window WHILE it is still being gated (streaming decode),
+// instead of starting when the window closes.
+constexpr unsigned kProgressPollNs = 300;
 struct ProgressWait {
   const volatile int* counter;
-  uint64_t* bell;
-  uint32_t seen;
 };
-__device__ __forceinline__ void progress_wait(ProgressWait* pw, int need)
+__device__ __forceinline__ void progress_wait(const ProgressWait* pw, int need)
 {
   if (!pw || !pw->counter) return;
-  while (*pw->counter < need) {
-    if (pw->bell) { if (mbar_try_wait_hint(pw->bell, pw->seen & 1u, 2000)) pw->seen++; }
-    else __nanosleep(RFID_B200_PROGRESS_NS);
-  }
+  while (*pw->counter < need) __nanosleep(kProgressPollNs);
   asm volatile("fence.acq_rel.cta;" ::: "memory");  // the samples were written (and fenced, CTA scope) before the counter moved
 }
 
-// dc: subtracted from every sample as it is staged (x - (+0.0f) == x for every x, so the default changes nothing).
+// dc: subtracted from every sample as it is staged (x - (+0.0f) == x for every x: a window that holds w already passes 0).
 // All loads of a fill are issued before the first store (kFillBatch per lane): the fill costs one trip to L2, not one per
 // 32 samples.
 // Where a window lives in global memory: sample g of the window is base[(ofs + g) & mask].  mask = -1: a plain array; the
@@ -114,7 +101,7 @@ __device__ __forceinline__ float l1_touch_span(const WinSrc gw, int lo, int coun
   return d;
 }
 __device__ __forceinline__ void stage_fill(float2* stage, const WinSrc gw, int lo, int count, int n_avail,
-                                           ProgressWait* progress = nullptr, float2 dc = make_float2(0.f, 0.f))
+                                           const ProgressWait* progress, float2 dc)
 {
   const int lane = threadIdx.x & 31;
   __syncwarp();
@@ -135,21 +122,17 @@ __device__ __forceinline__ void stage_fill(float2* stage, const WinSrc gw, int l
   __syncwarp();
 }
 
-// same, storing |w|^2 (std::norm: re*re + im*im, separately rounded) instead of the sample
-// L1: load through the SM's L1 (ld.global.ca) instead of L2 only -- for callers that touched the lines beforehand
-template <bool L1 = false>
-__device__ __forceinline__ void stage_fill_norm(float* stage_m, const WinSrc gw, int lo, int count, int n_avail,
-                                                ProgressWait* progress = nullptr, float2 dc = make_float2(0.f, 0.f))
+// same, storing |w|^2 (std::norm: re*re + im*im, separately rounded) instead of the sample; the range must be present
+__device__ __forceinline__ void stage_fill_norm(float* stage_m, const WinSrc gw, int lo, int count, int n_avail, float2 dc)
 {
   const int lane = threadIdx.x & 31;
   __syncwarp();
-  progress_wait(progress, min(n_avail, lo + count));
   for (int p0 = 0; p0 < count; p0 += 32 * kFillBatch) {
     float2 v[kFillBatch];
 #pragma unroll
     for (int k = 0; k < kFillBatch; k++) {
       const int p = p0 + 32 * k + lane, g = lo + p;
-      v[k] = (p < count && g >= 0 && g < n_avail) ? (L1 ? ld_ca_f2(gw.at(g)) : __ldcg(gw.at(g))) : make_float2(0.f, 0.f);
+      v[k] = (p < count && g >= 0 && g < n_avail) ? __ldcg(gw.at(g)) : make_float2(0.f, 0.f);
     }
 #pragma unroll
     for (int k = 0; k < kFillBatch; k++) {
@@ -163,8 +146,7 @@ __device__ __forceinline__ void stage_fill_norm(float* stage_m, const WinSrc gw,
 // Whole window present (nobody to wait for): optionally touch the span's cache lines (L2 -> this SM's L1, one load per
 // lane), then fill in rolled batches of four loads per lane through L1.  Small code, and one trip to L2 per fill.  The
 // window was written by this SM before the decode began; an SM's own stores keep its L1 coherent.
-template <bool NORM>
-__device__ __forceinline__ void stage_fill_l1(void* stage_v, const WinSrc gw, int lo, int count, int n_avail, float2 dc, bool touch)
+__device__ __forceinline__ void stage_fill_l1(float2* stage, const WinSrc gw, int lo, int count, int n_avail, float2 dc, bool touch)
 {
   const int lane = threadIdx.x & 31;
   __syncwarp();
@@ -181,11 +163,7 @@ __device__ __forceinline__ void stage_fill_l1(void* stage_v, const WinSrc gw, in
 #pragma unroll
     for (int k = 0; k < 4; k++) {
       const int p = p0 + 32 * k + lane, g = lo + p;
-      const bool in = g >= 0 && g < n_avail;
-      if (p < count) {
-        if (NORM) reinterpret_cast<float*>(stage_v)[p] = in ? c_norm(c_sub(v[k], dc)) : 0.0f;
-        else reinterpret_cast<float2*>(stage_v)[p] = in ? c_sub(v[k], dc) : make_float2(0.f, 0.f);
-      }
+      if (p < count) stage[p] = (g >= 0 && g < n_avail) ? c_sub(v[k], dc) : make_float2(0.f, 0.f);
     }
   }
   asm volatile("" ::"f"(sink));
@@ -197,7 +175,7 @@ __device__ __forceinline__ void stage_fill_l1(void* stage_v, const WinSrc gw, in
 // finish (argmax, 128 bit decisions :171-191, CRC).  Each phase needs the window only up to a known position, so a
 // caller that is still receiving the window (rx_pack.cuh: warp C copies it tile by tile) runs the phases as the samples
 // arrive; decode_window_staged below runs them back to back.  One copy of the arithmetic either way.
-constexpr int kChunkSteps = 64;                       // steps of the symbol-period search per phase (one stage fill each)
+constexpr int kChunkSteps = 64;                       // steps of the symbol-period search per phase
 constexpr int kSearchChunks = 256 / kChunkSteps;
 struct WinStream {
   int phase;     // 0: head pending, 1..kSearchChunks: search chunk (phase - 1) pending, kSearchChunks + 1: search complete
@@ -221,12 +199,22 @@ __device__ __forceinline__ int win_head_samples(const RxConfig& c, int kind, int
   return min(stage_cap, kind == RFID_B200_RN16 ? n_total : (int)(c.sync_range + 6.0f * c.n_tag_bit_f) + 2);
 }
 
-// window samples a search chunk reads (exclusive upper bound, clamped to the window)
-__device__ __forceinline__ int win_chunk_need(const RxConfig& c, const WinStream& S, int chunk, int n_total, int stage_cap)
+// Samples a search chunk reads, from the smallest index any candidate touches in it (win_chunk_lo): kChunkSteps steps at
+// the longest candidate period, plus how far the longest candidate has drifted from the shortest by the last chunk, plus
+// slack.  Also the host's decoder-stage rule (rfid_b200.cu), so host and device agree on which stages hold a chunk.
+__host__ __device__ inline int win_chunk_span(const RxConfig& c)
 {
-  const int span = min(2 * stage_cap, (int)((float)kChunkSteps * c.t_max + 256.0f * (c.t_max - c.t_min)) + 8);
-  const int lo = (int)f_add(f_mul((float)(kChunkSteps * chunk), c.t_min), (float)S.index);
-  return min(n_total, lo + span);
+  return (int)((float)kChunkSteps * c.t_max + 256.0f * (c.t_max - c.t_min)) + 8;
+}
+__device__ __forceinline__ int win_chunk_lo(const RxConfig& c, int index, int chunk)
+{
+  return (int)f_add(f_mul((float)(kChunkSteps * chunk), c.t_min), (float)index);
+}
+
+// window samples a search chunk reads (exclusive upper bound, clamped to the window)
+__device__ __forceinline__ int win_chunk_need(const RxConfig& c, int index, int chunk, int n_total)
+{
+  return min(n_total, win_chunk_lo(c, index, chunk) + win_chunk_span(c));
 }
 
 // tag_sync + h_est; fills sync_index / score / h of `out` and the stream state.  progress = null: the whole window is
@@ -234,14 +222,14 @@ __device__ __forceinline__ int win_chunk_need(const RxConfig& c, const WinStream
 // window is still being written -- the head is loaded through L2 only, so that L1 keeps no line of the unwritten part.
 __device__ __forceinline__ void win_stream_head(const RxConfig& c, int kind, const WinSrc gw, int n_total,
                                                 float2* __restrict__ stage, int stage_cap, float2 dc, WinStream& S,
-                                                WindowDecode& out, ProgressWait* progress = nullptr)
+                                                WindowDecode& out, const ProgressWait* progress = nullptr)
 {
   const int lane = threadIdx.x & 31;
   const float n = c.n_tag_bit_f;
   const float half = f_mul(n, 0.5f);   // (x / 2 == x * 0.5 exactly, every x)
   const int head = win_head_samples(c, kind, n_total, stage_cap);
   if (progress) stage_fill(stage, gw, 0, head, n_total, progress, dc);
-  else stage_fill_l1<false>(stage, gw, 0, head, n_total, dc, true);
+  else stage_fill_l1(stage, gw, 0, head, n_total, dc, true);
   // (whole window present: start the first search chunk's lines towards L1 now; it begins 6.5 symbols after the sync index)
   float sink = 0.0f;
   if (!progress && kind != RFID_B200_RN16) sink = l1_touch_span(gw, (int)(6.5f * n), 32 * 16, n_total);
@@ -292,39 +280,56 @@ __device__ __forceinline__ void win_stream_head(const RxConfig& c, int kind, con
   asm volatile("" ::"f"(sink));
 }
 
-// kChunkSteps steps of the symbol-period search: E_t += M[(int)(i * T_t + index)], i ascending
+// One chunk (kChunkSteps steps) of the symbol-period search: E_t += M[(int)(i * T_t + index)], i ascending, eight gathers
+// in flight and then their eight additions in order.  Only M = |w|^2 is needed (magn_squared_samples,
+// gate_impl.cc:176,186).  STAGED: the kernel's stage holds a chunk's span at one float per sample (rfid_b200.cu,
+// chunk_stage_samples); it is filled with M and the steps gather from there.  Else (rx_fused_kernel, whose stage holds
+// the head only) the steps gather the samples straight from L2.  The source is fixed per kernel at compile time: a kernel
+// that carries both loops pays in registers for the one it never runs (spills in its other roles; rx_fused_kernel took
+// 2-5 % longer at 4-8 MS/s on an H100 SXM at a 400 W power limit).
+template <bool STAGED>
 __device__ __forceinline__ void win_stream_chunk(const RxConfig& c, const WinSrc gw, int n_total,
                                                  float2* __restrict__ stage, int stage_cap, float2 dc, WinStream& S,
-                                                 ProgressWait* progress = nullptr)
+                                                 const ProgressWait* progress = nullptr)
 {
   const int lane = threadIdx.x & 31;
   const int number_steps = 20;
-  const int chunk = S.phase - 1;
-  const int i0 = kChunkSteps * chunk;
-  // Only |w|^2 is needed here (magn_squared_samples, gate_impl.cc:176,186), so the stage holds one float per sample.
+  const int i0 = kChunkSteps * (S.phase - 1);
+  const int span = win_chunk_span(c);
+  const int lo = win_chunk_lo(c, S.index, S.phase - 1);
   float* stage_m = reinterpret_cast<float*>(stage);
-  const int span = min(2 * stage_cap, (int)((float)kChunkSteps * c.t_max + 256.0f * (c.t_max - c.t_min)) + 8);
-  const int lo = (int)f_add(f_mul((float)i0, c.t_min), (float)S.index);  // smallest index any candidate touches
-  stage_fill_norm(stage_m, gw, lo, span, n_total, progress, dc);
+  progress_wait(progress, min(n_total, lo + span));
+  if (STAGED) {
+    if (span > 2 * stage_cap) __trap();   // a stage below the host's rule: fail rather than read stale entries
+    stage_fill_norm(stage_m, gw, lo, span, n_total, dc);
+  }
   if (lane < number_steps) {
     const float findex = (float)S.index, Tt = S.Tt;
-    float fi = (float)i0;                          // (float)i, advanced by exact +1.0f steps
     float e = S.e;
-#pragma unroll 8
-    for (int i = i0; i < i0 + kChunkSteps; i++) {
-      const int p = (int)f_add(f_mul(fi, Tt), findex);  // (int)(i * T + index), :161; fi == (float)i exactly
-      e = f_add(e, stage_m[p - lo]);
-      fi = f_add(fi, 1.0f);
+#pragma unroll 1
+    for (int i = i0; i < i0 + kChunkSteps; i += 8) {
+      const float fi = (float)i;
+      float2 g[8];                                   // STAGED: M in .x; else the sample (dc outside the window)
+      bool in[8];
+#pragma unroll
+      for (int u = 0; u < 8; u++) {
+        const int p = (int)f_add(f_mul(f_add(fi, (float)u), Tt), findex);  // (int)(i * T + index), :161 (exact: i < 256)
+        in[u] = p >= 0 && p < n_total;
+        if (STAGED) g[u].x = stage_m[p - lo];
+        else g[u] = in[u] ? __ldcg(gw.at(p)) : dc;
+      }
+#pragma unroll
+      for (int u = 0; u < 8; u++) e = f_add(e, STAGED ? g[u].x : in[u] ? c_norm(c_sub(g[u], dc)) : 0.0f);
     }
     S.e = e;
   }
   S.phase++;
 }
 
-// EPC, the symbol-period search complete: argmax, 128 bit decisions, CRC-16 (the end of win_stream_finish)
-__device__ __forceinline__ void win_stream_decide(const RxConfig& c, const WinSrc gw, int n_avail, float2* __restrict__ stage,
-                                                  int stage_cap, float2 dc, const WinStream& S, WindowDecode& out,
-                                                  ProgressWait* progress = nullptr, long long* pp = nullptr)
+// EPC, the symbol-period search complete: argmax, 128 bit decisions, CRC-16 (the end of win_stream_finish).  The whole
+// window must be present.
+__device__ __forceinline__ void win_stream_decide(const RxConfig& c, const WinSrc gw, int n_avail, float2 dc,
+                                                  const WinStream& S, WindowDecode& out, long long* pp)
 {
   const int lane = threadIdx.x & 31;
   const int index = S.index;
@@ -338,43 +343,27 @@ __device__ __forceinline__ void win_stream_decide(const RxConfig& c, const WinSr
   const int index_T = e_idx;
   const float T = f_add(min_val, f_div(f_mul((float)index_T, f_sub(max_val, min_val)), (float)(number_steps - 1)));
   out.T = T;
-  // ---- 128 bit decisions (:171-191), 32 pairs per stage fill
+  // ---- 128 bit decisions (:171-191): every lane gathers its eight samples straight from L2, all loads in flight
+  // together (outside the window a sample is 0, as a stage fill makes it)
   const float twoT = f_mul(2.0f, T);
+  float2 wa[4], wb[4];
+  bool ia[4], ib[4];
+#pragma unroll
+  for (int r = 0; r < 4; r++) {
+    const int j = r * 32 + lane;
+    const int a = (int)f_add(f_mul((float)j, twoT), (float)index);
+    const int b = (int)f_add(f_add(f_mul((float)(j * 2), T), T), (float)index);
+    ia[r] = a >= 0 && a < n_avail;
+    ib[r] = b >= 0 && b < n_avail;
+    wa[r] = ia[r] ? __ldcg(gw.at(a)) : dc;
+    wb[r] = ib[r] ? __ldcg(gw.at(b)) : dc;
+  }
   unsigned Sg[4];
-  if (!progress) {
-    // the whole window is present: every lane gathers its eight samples straight from L2, all loads in flight together
-    float2 wa[4], wb[4];
 #pragma unroll
-    for (int r = 0; r < 4; r++) {
-      const int j = r * 32 + lane;
-      const int a = (int)f_add(f_mul((float)j, twoT), (float)index);
-      const int b = (int)f_add(f_add(f_mul((float)(j * 2), T), T), (float)index);
-      const bool ia = a >= 0 && a < n_avail, ib = b >= 0 && b < n_avail;   // (outside the window: 0, as the stage fill does)
-      wa[r] = ia ? __ldcg(gw.at(a)) : dc;
-      wb[r] = ib ? __ldcg(gw.at(b)) : dc;
-    }
-#pragma unroll
-    for (int r = 0; r < 4; r++) {
-      const int j = r * 32 + lane;
-      const int a = (int)f_add(f_mul((float)j, twoT), (float)index);
-      const int b = (int)f_add(f_add(f_mul((float)(j * 2), T), T), (float)index);
-      const float2 sa = (a >= 0 && a < n_avail) ? c_sub(wa[r], dc) : make_float2(0.f, 0.f);
-      const float2 sb = (b >= 0 && b < n_avail) ? c_sub(wb[r], dc) : make_float2(0.f, 0.f);
-      const float res = c_proj(sa, sb, h);
-      Sg[r] = __ballot_sync(0xffffffffu, res > 0.0f);
-    }
-  } else {
-#pragma unroll
-    for (int r = 0; r < 4; r++) {
-      const int j0 = r * 32;
-      const int lo = (int)f_add(f_mul((float)j0, twoT), (float)index);
-      stage_fill(stage, gw, lo, stage_cap, n_avail, progress, dc);
-      int j = j0 + lane;
-      int a = (int)f_add(f_mul((float)j, twoT), (float)index);
-      int b = (int)f_add(f_add(f_mul((float)(j * 2), T), T), (float)index);
-      float res = c_proj(stage[a - lo], stage[b - lo], h);
-      Sg[r] = __ballot_sync(0xffffffffu, res > 0.0f);
-    }
+  for (int r = 0; r < 4; r++) {
+    const float2 sa = ia[r] ? c_sub(wa[r], dc) : make_float2(0.f, 0.f);
+    const float2 sb = ib[r] ? c_sub(wb[r], dc) : make_float2(0.f, 0.f);
+    Sg[r] = __ballot_sync(0xffffffffu, c_proj(sa, sb, h) > 0.0f);
   }
   if (pp && lane == 0) pp[3] = clock64();
   unsigned carry = 1u;
@@ -390,11 +379,13 @@ __device__ __forceinline__ void win_stream_decide(const RxConfig& c, const WinSr
   if (pp && lane == 0) pp[4] = clock64();
 }
 
-// RN16: half-bit sampling + tag_detection_RN16 (:114-142, :237-253); EPC: remaining search chunks, argmax, 128 bit
-// decisions, CRC-16.  The whole window must be present.
+// RN16: half-bit sampling + tag_detection_RN16 (:114-142, :237-253); the whole window must be present.  EPC: remaining
+// search chunks (each waits for the samples it reads), then, the whole window present, argmax, 128 bit decisions, CRC-16.
+template <bool STAGED>
 __device__ __forceinline__ void win_stream_finish(const RxConfig& c, int kind, const WinSrc gw, int n_avail,
                                                   float2* __restrict__ stage, int stage_cap, float2 dc, WinStream& S,
-                                                  WindowDecode& out, ProgressWait* progress = nullptr, long long* pp = nullptr)
+                                                  WindowDecode& out, const ProgressWait* progress = nullptr,
+                                                  long long* pp = nullptr)
 {
   const int lane = threadIdx.x & 31;
   const float n = c.n_tag_bit_f;
@@ -433,108 +424,25 @@ __device__ __forceinline__ void win_stream_finish(const RxConfig& c, int kind, c
     if (pp && lane == 0) { pp[2] = pp[3] = pp[4] = clock64(); }
     return;
   }
-  if (!progress) {
-    // ---- remaining chunks of the symbol-period search, whole window present (nobody to wait for): while chunk k's 64
-    // steps run from the stage, chunk k+1's samples travel from L2 into registers; 16 gathers in flight, added in order.
-    // (Tried: all 32 lanes gathering 16 steps x 20 candidates into a table that lane t then adds up in order -- fewer
-    // instructions, but slower than the plain loop below: 19.6 k vs 15.6 k cycles per window.)
-    float* stage_m = reinterpret_cast<float*>(stage);
-    const int span_full = (int)((float)kChunkSteps * c.t_max + 256.0f * (c.t_max - c.t_min)) + 8;
-    const int span = min(2 * stage_cap, span_full);
-    if (span_full > 2 * stage_cap || span > 32 * kFillBatch) {
-      // the stage holds the head only (kernels whose shared memory is spoken for), or a chunk is longer than one load
-      // batch: |w|^2 straight from global memory, eight gathers in flight, added in order
-      if (lane < 20) {
-        const float findex = (float)index, Tt = S.Tt;
-        float e = S.e;
-#pragma unroll 1
-        for (int i = kChunkSteps * (S.phase - 1); i < kChunkSteps * kSearchChunks; i += 8) {
-          const float fi = (float)i;
-          float2 g8[8];
-          bool in8[8];
-#pragma unroll
-          for (int u = 0; u < 8; u++) {
-            const int p = (int)f_add(f_mul(f_add(fi, (float)u), Tt), findex);  // (int)(i * T + index), :161
-            in8[u] = p >= 0 && p < n_avail;
-            g8[u] = in8[u] ? __ldcg(gw.at(p)) : dc;
-          }
-#pragma unroll
-          for (int u = 0; u < 8; u++) e = f_add(e, in8[u] ? c_norm(c_sub(g8[u], dc)) : 0.0f);
-        }
-        S.e = e;
-      }
-      S.phase = kSearchChunks + 1;
-    } else {
-      // chunk k+1's samples travel from L2 into registers while chunk k's 64 steps run from the stage
-      float2 v[kFillBatch];
-      int lo = (int)f_add(f_mul((float)(kChunkSteps * (S.phase - 1)), c.t_min), (float)index);
-      auto issue = [&](int lo_) {
-#pragma unroll
-        for (int k = 0; k < kFillBatch; k++) {
-          const int p = 32 * k + lane, g = lo_ + p;
-          v[k] = (p < span && g >= 0 && g < n_avail) ? __ldcg(gw.at(g)) : make_float2(0.f, 0.f);
-        }
-      };
-      issue(lo);
-      while (S.phase <= kSearchChunks) {
-        const int i0 = kChunkSteps * (S.phase - 1);
-        __syncwarp();  // the previous chunk's reads of the stage are complete
-#pragma unroll
-        for (int k = 0; k < kFillBatch; k++) {
-          const int p = 32 * k + lane, g = lo + p;
-          if (p < span) stage_m[p] = (g >= 0 && g < n_avail) ? c_norm(c_sub(v[k], dc)) : 0.0f;
-        }
-        __syncwarp();
-        const float* sm = stage_m - lo;
-        if (S.phase < kSearchChunks) {
-          lo = (int)f_add(f_mul((float)(i0 + kChunkSteps), c.t_min), (float)index);
-          issue(lo);
-        }
-        if (lane < 20) {
-          const float findex = (float)index, Tt = S.Tt;
-          float e = S.e;
-#pragma unroll 1
-          for (int i = i0; i < i0 + kChunkSteps; i += 16) {
-            // sixteen gathers in flight, then their sixteen additions in order
-            const float fi = (float)i;
-            float u16[16];
-#pragma unroll
-            for (int u = 0; u < 16; u++) u16[u] = sm[(int)f_add(f_mul(f_add(fi, (float)u), Tt), findex)];  // (int)(i * T + index), :161
-#pragma unroll
-            for (int u = 0; u < 16; u++) e = f_add(e, u16[u]);
-          }
-          S.e = e;
-        }
-        S.phase++;
-      }
-      __syncwarp();
-    }
-  } else {
-    while (S.phase <= kSearchChunks) win_stream_chunk(c, gw, n_avail, stage, stage_cap, dc, S, progress);
-  }
-  win_stream_decide(c, gw, n_avail, stage, stage_cap, dc, S, out, progress, pp);
+  while (S.phase <= kSearchChunks) win_stream_chunk<STAGED>(c, gw, n_avail, stage, stage_cap, dc, S, progress);
+  progress_wait(progress, n_avail);
+  win_stream_decide(c, gw, n_avail, dc, S, out, pp);
 }
 
-__device__ __forceinline__ void decode_window_staged(const RxConfig& c, int kind, const WinSrc gw, int n_avail,
-                                                     float2* __restrict__ stage, int stage_cap, WindowDecode& out,
-                                                     const volatile int* progress_counter = nullptr, uint64_t* bell = nullptr,
-                                                     float2 dc = make_float2(0.f, 0.f), long long* pp = nullptr)
-{
-  ProgressWait pw_{progress_counter, bell, 0u};
-  ProgressWait* const progress = progress_counter ? &pw_ : nullptr;
-  WinStream S;
-  if (pp && (threadIdx.x & 31) == 0) pp[0] = clock64();
-  win_stream_head(c, kind, gw, n_avail, stage, stage_cap, dc, S, out, progress);
-  if (pp && (threadIdx.x & 31) == 0) pp[1] = clock64();
-  win_stream_finish(c, kind, gw, n_avail, stage, stage_cap, dc, S, out, progress, pp);
-}
-
+// The decode of one window held in w[0, n_avail), its phases back to back.  progress_counter (may be null): window
+// samples published so far, for a window that is still being gated.  STAGED: as win_stream_chunk.
+template <bool STAGED>
 __device__ __forceinline__ void decode_window_staged(const RxConfig& c, int kind, const float2* __restrict__ w, int n_avail,
                                                      float2* __restrict__ stage, int stage_cap, WindowDecode& out,
-                                                     const volatile int* progress_counter = nullptr, uint64_t* bell = nullptr,
-                                                     float2 dc = make_float2(0.f, 0.f))
+                                                     const volatile int* progress_counter = nullptr)
 {
-  decode_window_staged(c, kind, WinSrc{w, 0, -1}, n_avail, stage, stage_cap, out, progress_counter, bell, dc);
+  const WinSrc gw{w, 0, -1};
+  const float2 dc = make_float2(0.f, 0.f);
+  const ProgressWait pw{progress_counter};
+  const ProgressWait* const progress = progress_counter ? &pw : nullptr;
+  WinStream S;
+  win_stream_head(c, kind, gw, n_avail, stage, stage_cap, dc, S, out, progress);
+  win_stream_finish<STAGED>(c, kind, gw, n_avail, stage, stage_cap, dc, S, out, progress);
 }
 
 __device__ __forceinline__ void store_result(rfid_b200_window_result* dst, const WindowDecode& d, int segment, int window,

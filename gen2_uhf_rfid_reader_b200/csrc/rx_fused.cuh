@@ -569,7 +569,7 @@ __global__ void __launch_bounds__(kFusedThreads, 8) rx_fused_kernel(const FusedA
       const int ordinal = B.meta_ordinal[j & 1], open_idx = B.meta_open[j & 1], len = B.meta_len[j & 1];
       WindowDecode wd;
       const float2* win = win_base + (kind ? A.rn16_pad : 0);
-      decode_window_staged(C, kind, win, len, dstage, A.dstage_samples, wd);
+      decode_window_staged<false>(C, kind, win, len, dstage, A.dstage_samples, wd);
       rfid_b200_window_result* dst = A.results + (size_t)seg * A.max_windows + ordinal;
       if (lane == 0) store_result(dst, wd, seg + A.seg_base, ordinal, open_idx, len, kind);
 #ifndef RFID_B200_PHASE_PROFILE

@@ -858,7 +858,7 @@ __global__ void __launch_bounds__(kSplitThreads, 7) rx_fused_split_kernel(const 
       const int ordinal = B.meta_ordinal[j & 1], open_idx = B.meta_open[j & 1], len = B.meta_len[j & 1];
       const float2* win = win_base + (kind ? A.rn16_pad : 0);
       WindowDecode wd;
-      decode_window_staged(C, kind, win, len, dstage, A.dstage_samples, wd, (const volatile int*)&B.progress[j & 1]);
+      decode_window_staged<true>(C, kind, win, len, dstage, A.dstage_samples, wd, (const volatile int*)&B.progress[j & 1]);
       rfid_b200_window_result* dst = A.results + (size_t)seg * A.max_windows + ordinal;
       const bool aborted = *(volatile int*)&B.aborted[j & 1] != 0;
       if (lane == 0 && !aborted) store_result(dst, wd, seg + A.seg_base, ordinal, open_idx, len, kind);

@@ -282,7 +282,7 @@ __device__ __forceinline__ void pack_decode_phase(const RxConfig& C, PackWinStat
   WindowDecode wd;
   if (phase == 0) {
     // the whole window present: the head through L1, as decode_window_staged; else through L2 only
-    ProgressWait l2_only{nullptr, nullptr, 0u};
+    const ProgressWait l2_only{nullptr};
     win_stream_head(C, kind, wv, len, dstage, stage_cap, dc, S, wd, act == 3 ? nullptr : &l2_only);
     if (pe && lane == 0) pe[1] = clock64();
   } else {
@@ -294,20 +294,12 @@ __device__ __forceinline__ void pack_decode_phase(const RxConfig& C, PackWinStat
   }
   if (act == 2) {
     const long long t = pe ? clock64() : 0;
-    win_stream_chunk(C, wv, len, dstage, stage_cap, dc, S);
+    win_stream_chunk<true>(C, wv, len, dstage, stage_cap, dc, S);
     if (pe && lane == 0) { pe[5] += clock64() - t; pe[7]++; }
   }
   if (act == 3) {
     if (pe && lane == 0) pe[6] = clock64();
-    if (kind == RFID_B200_RN16) {
-      win_stream_finish(C, kind, wv, len, dstage, stage_cap, dc, S, wd, nullptr, pe);
-    } else {
-      // chunk by chunk, not win_stream_finish's search: that one keeps the next chunk's samples in 24 registers while a
-      // chunk runs, which in this kernel (64 registers per thread) leaves ptxas none for the chunk's gathers -- every
-      // step became one dependent chain of index, gather and add.  Here a chunk's eight gathers are in flight together.
-      while (S.phase <= kSearchChunks) win_stream_chunk(C, wv, len, dstage, stage_cap, dc, S);
-      win_stream_decide(C, wv, len, dstage, stage_cap, dc, S, wd, nullptr, pe);
-    }
+    win_stream_finish<true>(C, kind, wv, len, dstage, stage_cap, dc, S, wd, nullptr, pe);
     if (lane == 0) store_result(dst, wd, seg_id, ord, wopen, len, kind);
     if (tap)
       for (int p2 = lane; p2 < len; p2 += 32) tap[p2] = c_sub(__ldcg(wv.at(p2)), dc);
@@ -1040,9 +1032,7 @@ __global__ void __launch_bounds__(kPackMaxThreads, 1) rx_pack_kernel(const PackA
             } else if (kind && phase == 0) {
               act = avail >= win_head_samples(C, kind, len, A.dstage_samples) ? 1 : 0;
             } else if (kind && phase <= kSearchChunks) {
-              WinStream ws;
-              ws.index = S.w.index;
-              act = avail >= win_chunk_need(C, ws, phase - 1, len, A.dstage_samples) ? 2 : 0;
+              act = avail >= win_chunk_need(C, S.w.index, phase - 1, len) ? 2 : 0;
             }
             if (act) key = (unsigned)(kind ? kSearchChunks + 3 - phase : 2) * 16u + 15u - (unsigned)lane;
           }
