@@ -254,7 +254,7 @@ __global__ void query_nsmid_kernel(unsigned* out)
 bool pack_ok(const RxConfig& c)
 {
   return c.decim == 5 && c.mf_rem == 0 && c.mf_q == 5 && fast_path_ok(c) && c.len_rn16 >= kT2 / 2 &&
-         c.len_epc + c.dc_length + 8 * kT2 <= kYW && ((c.win_length | c.dc_length) & 3) == 0 && c.dc_length <= 124 && c.win_length <= kT2 && c.n_T1 + 1 >= 32;
+         c.len_epc + c.dc_length + 8 * kT2 <= kYW && ((c.win_length | c.dc_length) & 3) == 0 && c.dc_length <= 124 && c.win_length <= kT2;
 }
 
 // shared-memory carve-up of rx_pack_kernel for G segments per CTA

@@ -1,6 +1,7 @@
 // rx_common.cuh -- shared definitions of the sm_90a Gen2 receive path:
 // derived configuration, the numerical contract (how each libm/libgcc call the
-// reference makes is evaluated on the device), mbarrier / TMA-bulk PTX wrappers.
+// reference makes is evaluated on the device), mbarrier / TMA-bulk PTX wrappers,
+// the capture kernels' raw-tile loader and running-sum replay.
 //
 // Numerical contract (SURVEY.md Appendix A.5; every item is exercised by the
 // parity tests against the compiled reference):
@@ -248,6 +249,110 @@ __device__ __forceinline__ void tma_load_1d_hint(void* smem_dst, const void* gme
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads)
 {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+
+// ---- what every capture kernel does with its tiles: raw-tile copies, running-sum replay ----
+constexpr int kTT = 128;          // decimated samples per tile (rx_pack_kernel: per half-tile)
+
+__device__ __forceinline__ void chain8(float4& u, float4& v, float& acc)
+{
+  acc = f_add(acc, u.x); u.x = acc;
+  acc = f_add(acc, u.y); u.y = acc;
+  acc = f_add(acc, u.z); u.z = acc;
+  acc = f_add(acc, u.w); u.w = acc;
+  acc = f_add(acc, v.x); v.x = acc;
+  acc = f_add(acc, v.y); v.y = acc;
+  acc = f_add(acc, v.z); v.z = acc;
+  acc = f_add(acc, v.w); v.w = acc;
+}
+
+// Sequential in-place running sum: acc = acc + buf[i]; buf[i] = acc (one rounding per step, the order of
+// the reference's recurrences).  The next 8 inputs are always in flight while 8 dependent adds retire, so
+// the loop runs at the FADD dependency latency.  May READ up to 16 floats past buf[n-1] (callers pad).
+__device__ __forceinline__ void chain_inplace(float* buf, int n, float& acc)
+{
+  int i = 0;
+  if (n >= 16) {
+    float4 a0 = *reinterpret_cast<const float4*>(buf), a1 = *reinterpret_cast<const float4*>(buf + 4);
+    for (; i + 16 <= n; i += 16) {
+      float4 b0 = *reinterpret_cast<const float4*>(buf + i + 8), b1 = *reinterpret_cast<const float4*>(buf + i + 12);
+      chain8(a0, a1, acc);
+      *reinterpret_cast<float4*>(buf + i) = a0;
+      *reinterpret_cast<float4*>(buf + i + 4) = a1;
+      a0 = *reinterpret_cast<const float4*>(buf + i + 16);
+      a1 = *reinterpret_cast<const float4*>(buf + i + 20);
+      chain8(b0, b1, acc);
+      *reinterpret_cast<float4*>(buf + i + 8) = b0;
+      *reinterpret_cast<float4*>(buf + i + 12) = b1;
+    }
+  }
+  for (; i < n; i++) {
+    acc = f_add(acc, buf[i]);
+    buf[i] = acc;
+  }
+}
+
+// raw tile geometry: segment-relative index of the first sample held in the stage buffer
+template <int DECIM>
+__device__ __forceinline__ long long tile_load_start(unsigned long long seg_off, int k)
+{
+  long long lo = (long long)DECIM * k * kTT - (DECIM - 1);
+  if (lo < 0) lo = 0;
+  long long abs_lo = (long long)seg_off + lo;
+  abs_lo &= ~1ll;  // 16-byte aligned source
+  return abs_lo - (long long)seg_off;
+}
+
+// the copy of raw tile k of segment sg (any tile; iq holds n_raw samples)
+template <int DECIM>
+__device__ __forceinline__ void issue_tile_load(const float2* iq, unsigned long long n_raw, const rfid_b200_segment& sg,
+                                                int k, float2* stage, uint64_t* bar)
+{
+  const long long start = tile_load_start<DECIM>(sg.offset, k);  // may be -1
+  long long hi = (long long)DECIM * ((long long)k * kTT + kTT - 1);
+  if (hi > (long long)sg.length - 1) hi = (long long)sg.length - 1;
+  long long count = hi - start + 1;  // samples start..hi
+  long long count_al = (count + 1) & ~1ll;
+  const long long abs_start = (long long)sg.offset + start;
+  float2 tail = make_float2(0.f, 0.f);
+  bool patch = false;
+  if ((unsigned long long)(abs_start + count_al) > n_raw) {
+    // the rounded-up copy would run one sample past the capture buffer: copy an even count and
+    // fetch the last sample with a plain load
+    count_al -= 2;
+    tail = iq[abs_start + count - 1];
+    patch = true;
+  }
+  const uint32_t bytes = (uint32_t)(count_al * 8);
+  if (patch) stage[count - 1] = tail;
+  mbar_arrive_expect_tx(bar, bytes);
+  if (bytes) tma_load_1d(stage, iq + abs_start, bytes, bar);
+}
+
+// Tile k >= 1 starts at raw sample D*kTT*k - (D-1) of the segment, moved down to an even absolute index (16-byte TMA
+// source); tile 0 starts at the segment's first (even-aligned) sample.  Tiles 1 .. n-1 are interior: their last sample
+// D*(k*kTT + kTT-1) exists and the rounded-up copy stays inside the capture, so each is `bytes` bytes from
+// src + D*kTT*k.  The other tiles go through issue_tile_load.
+struct InteriorTiles {
+  const float2* src;
+  uint32_t bytes;
+  int n;
+};
+template <int DECIM>
+__device__ __forceinline__ InteriorTiles interior_tiles(const float2* iq, unsigned long long n_raw,
+                                                        const rfid_b200_segment& sg, int ntiles)
+{
+  const int odd = (int)(sg.offset & 1ull);
+  InteriorTiles t;
+  t.src = iq + sg.offset - (DECIM - 1) - odd;
+  t.bytes = (uint32_t)((DECIM * kTT + 2 * odd) * 8);
+  const long long by_len = ((long long)sg.length - 1 - (long long)DECIM * (kTT - 1)) / ((long long)DECIM * kTT);
+  const long long room = (long long)n_raw - (long long)sg.offset + (DECIM - 1) + odd - (DECIM * kTT + 2 * odd);
+  const long long by_buf = room >= 0 ? room / ((long long)DECIM * kTT) : -1;
+  long long f = (by_len < by_buf ? by_len : by_buf) + 1;
+  if (sg.length < (unsigned)(DECIM * kTT)) f = 0;
+  t.n = f < 0 ? 0 : (f > ntiles ? ntiles : (int)f);
+  return t;
 }
 
 }  // namespace rfid_b200

@@ -15,7 +15,7 @@
 //               (gate_impl.cc:131), lanes 1,2: dc_est.re/.im over the closed samples of tile k-1
 //               (gate_impl.cc:141) -- then finishes tile k-1 (window emission with the now-known DC
 //               estimate, window hand-off to the decoder) and runs thresholds + the edge/pulse state
-//               machine of tile k as bit-mask hopping (a few steps per reader command).
+//               machine of tile k (rx_gate.cuh) on its 128-bit masks.
 //   workers x2  wait for the TMA bulk copy of the next raw tile, block-sum matched filter, |y|
 //               (exact cabsf), amplitude-ring difference / win_length  -> tile stage.
 //   decoder     decodes each closed window from shared memory (preamble correlation, channel
@@ -26,6 +26,7 @@
 
 #include "rx_common.cuh"
 #include "rx_decode.cuh"
+#include "rx_gate.cuh"
 
 namespace rfid_b200 {
 
@@ -40,7 +41,6 @@ namespace rfid_b200 {
 #define PH_DUMP(base)
 #endif
 
-constexpr int kTT = 128;          // decimated samples per tile
 constexpr int kRawStages = 2;
 constexpr int kTileStages = 3;    // >= 3: tile k-1 is still being finished while tile k+1 is produced
 constexpr int kWorkerWarps = 2;
@@ -115,97 +115,9 @@ struct FusedShared {
   TileEvent ev[kMaxTileEvents];
 };
 
-__device__ __forceinline__ int next_set128(unsigned long long lo, unsigned long long hi, int pos)
-{
-  if (pos < 64) {
-    unsigned long long m = lo & (~0ull << pos);
-    if (m) return __ffsll((long long)m) - 1;
-    pos = 64;
-  }
-  if (pos < 128) {
-    unsigned long long m = hi & (~0ull << (pos - 64));
-    if (m) return 64 + __ffsll((long long)m) - 1;
-  }
-  return 128;
-}
-
-__device__ __forceinline__ void chain8(float4& u, float4& v, float& acc)
-{
-  acc = f_add(acc, u.x); u.x = acc;
-  acc = f_add(acc, u.y); u.y = acc;
-  acc = f_add(acc, u.z); u.z = acc;
-  acc = f_add(acc, u.w); u.w = acc;
-  acc = f_add(acc, v.x); v.x = acc;
-  acc = f_add(acc, v.y); v.y = acc;
-  acc = f_add(acc, v.z); v.z = acc;
-  acc = f_add(acc, v.w); v.w = acc;
-}
-
-// Sequential in-place running sum: acc = acc + buf[i]; buf[i] = acc (one rounding per step, the order of
-// the reference's recurrences).  The next 8 inputs are always in flight while 8 dependent adds retire, so
-// the loop runs at the FADD dependency latency.  May READ up to 16 floats past buf[n-1] (callers pad).
-__device__ __forceinline__ void chain_inplace(float* buf, int n, float& acc)
-{
-  int i = 0;
-  if (n >= 16) {
-    float4 a0 = *reinterpret_cast<const float4*>(buf), a1 = *reinterpret_cast<const float4*>(buf + 4);
-    for (; i + 16 <= n; i += 16) {
-      float4 b0 = *reinterpret_cast<const float4*>(buf + i + 8), b1 = *reinterpret_cast<const float4*>(buf + i + 12);
-      chain8(a0, a1, acc);
-      *reinterpret_cast<float4*>(buf + i) = a0;
-      *reinterpret_cast<float4*>(buf + i + 4) = a1;
-      a0 = *reinterpret_cast<const float4*>(buf + i + 16);
-      a1 = *reinterpret_cast<const float4*>(buf + i + 20);
-      chain8(b0, b1, acc);
-      *reinterpret_cast<float4*>(buf + i + 8) = b0;
-      *reinterpret_cast<float4*>(buf + i + 12) = b1;
-    }
-  }
-  for (; i < n; i++) {
-    acc = f_add(acc, buf[i]);
-    buf[i] = acc;
-  }
-}
-
-// raw tile geometry: segment-relative index of the first sample held in the stage buffer
-template <int DECIM>
-__device__ __forceinline__ long long tile_load_start(unsigned long long seg_off, int k)
-{
-  long long lo = (long long)DECIM * k * kTT - (DECIM - 1);
-  if (lo < 0) lo = 0;
-  long long abs_lo = (long long)seg_off + lo;
-  abs_lo &= ~1ll;  // 16-byte aligned source
-  return abs_lo - (long long)seg_off;
-}
-
-template <int DECIM>
-__device__ __forceinline__ void issue_tile_load(const FusedArgs& A, const rfid_b200_segment& sg, int k, float2* stage,
-                                                uint64_t* bar)
-{
-  const long long start = tile_load_start<DECIM>(sg.offset, k);  // may be -1
-  long long hi = (long long)DECIM * ((long long)k * kTT + kTT - 1);
-  if (hi > (long long)sg.length - 1) hi = (long long)sg.length - 1;
-  long long count = hi - start + 1;  // samples start..hi
-  long long count_al = (count + 1) & ~1ll;
-  const long long abs_start = (long long)sg.offset + start;
-  float2 tail = make_float2(0.f, 0.f);
-  bool patch = false;
-  if ((unsigned long long)(abs_start + count_al) > A.n_raw) {
-    // the rounded-up copy would run one sample past the capture buffer: copy an even count and
-    // fetch the last sample with a plain load
-    count_al -= 2;
-    tail = A.iq[abs_start + count - 1];
-    patch = true;
-  }
-  const uint32_t bytes = (uint32_t)(count_al * 8);
-  if (patch) stage[count - 1] = tail;
-  mbar_arrive_expect_tx(bar, bytes);
-  if (bytes) tma_load_1d(stage, A.iq + abs_start, bytes, bar);
-}
-
 // MFQ > 0: ntaps == MFQ * DECIM (compile-time unrolled block sums); MFQ == 0: generic ntaps.
-// This kernel keeps explicit amplitude / closed-sample rings of any length (raw rates above 5 MS/s, where the
-// reference's 250 us / 120 us windows are longer than a tile); rx_fused_split_kernel is the fast path below that.
+// This kernel keeps explicit amplitude / closed-sample rings of any length: it serves every rate whose 250 us window is
+// longer than a tile (raw rates of 2.6 MS/s and up); rx_fused_split_kernel is the fast path below that.
 template <int DECIM, int MFQ>
 __global__ void __launch_bounds__(kFusedThreads, 8) rx_fused_kernel(const FusedArgs A)
 {
@@ -253,7 +165,7 @@ __global__ void __launch_bounds__(kFusedThreads, 8) rx_fused_kernel(const FusedA
     const int wt = (warp - 1) * 32 + lane;
     if (wt == 0) {
       for (int k = 0; k < kRawStages && k < ntiles; k++)
-        issue_tile_load<DECIM>(A, sg, k, raw + (size_t)k * A.raw_stage_samples, &B.raw_full[k]);
+        issue_tile_load<DECIM>(A.iq, A.n_raw, sg, k, raw + (size_t)k * A.raw_stage_samples, &B.raw_full[k]);
     }
     const int bmask = A.bhist_size - 1, amask = A.ahist_size - 1;
     const float winlen_f = (float)C.win_length;
@@ -302,7 +214,7 @@ __global__ void __launch_bounds__(kFusedThreads, 8) rx_fused_kernel(const FusedA
       PH_MARK(2)
       bar_sync_workers();  // raw stage rs fully consumed, block sums visible
       if (wt == 0 && k + kRawStages < ntiles)
-        issue_tile_load<DECIM>(A, sg, k + kRawStages, raw + (size_t)rs * A.raw_stage_samples, &B.raw_full[rs]);
+        issue_tile_load<DECIM>(A.iq, A.n_raw, sg, k + kRawStages, raw + (size_t)rs * A.raw_stage_samples, &B.raw_full[rs]);
       PH_MARK(3)
       if (k >= kTileStages) bar_sync_stage<BAR_TILE_EMPTY>(ts, 96);  // the sequencer is done with tile k - 3
       PH_MARK(4)
@@ -360,8 +272,7 @@ __global__ void __launch_bounds__(kFusedThreads, 8) rx_fused_kernel(const FusedA
     // =========================================================== sequencer
     float acc = 0.f;  // lane 0: avg_ampl, lane 1: dc_est.re, lane 2: dc_est.im
     // --- gate state machine (runs one tile ahead of the window emission)
-    bool sig_pos = false;          // signal_state, starts NEG_EDGE (gate_impl.cc:45)
-    int n_samples = 0, num_pulses = 0;
+    GateFsm gs = {false, 0, 0};    // signal_state starts NEG_EDGE (gate_impl.cc:45)
     bool gate_open = false;
     int to_ungate = C.len_rn16;    // first SEEK is for an RN16 (global_vars.cc:47, reader_impl.cc:262)
     int wcount = 0;
@@ -453,42 +364,18 @@ __global__ void __launch_bounds__(kFusedThreads, 8) rx_fused_kernel(const FusedA
       if (k < ntiles && !terminated) {
         const float* ta = tile_a + ts * kTT;
         const float2* ty = tile_y + ts * kTT;
-        unsigned lt[4], gt[4];
-#pragma unroll
-        for (int r = 0; r < 4; r++) {
-          const int i = r * 32 + lane;
-          const bool v = i < nvalid;
-          const float thr = v ? f_mul(davg[i], kThreshFraction) : 0.f;  // gate_impl.cc:136
-          const float a = v ? ta[i] : 0.f;
-          lt[r] = __ballot_sync(0xffffffffu, v && a < thr);
-          gt[r] = __ballot_sync(0xffffffffu, v && a > thr);
-        }
-        const unsigned long long LT_lo = lt[0] | ((unsigned long long)lt[1] << 32), LT_hi = lt[2] | ((unsigned long long)lt[3] << 32);
-        const unsigned long long GT_lo = gt[0] | ((unsigned long long)gt[1] << 32), GT_hi = gt[2] | ((unsigned long long)gt[3] << 32);
+        unsigned ltw, gtw;   // word (lane & 3) of the threshold masks
+        gate_masks<4>(davg, ta, nvalid, ltw, gtw);
         PH_MARK(4)
 
         int pos = 0;
         while (pos < nvalid) {
           if (!gate_open) {
-            // ---- closed: hop from edge to edge (gate_impl.cc:145-162) until the tile ends or the gate opens
+            // ---- closed: edges, pulse counting and the open test of this run (gate_impl.cc:145-180)
             const int run_start = pos;
-            bool opened = false;
-            while (pos < nvalid) {
-              if (sig_pos) {
-                const int p_fall = next_set128(LT_lo, LT_hi, pos);
-                int p_open = 1 << 30;
-                if (num_pulses > kNumPulsesCommand) p_open = pos + max(0, C.n_T1 - n_samples);
-                if (p_fall >= nvalid && p_open >= nvalid) { n_samples += nvalid - pos; pos = nvalid; break; }
-                if (p_fall <= p_open) { n_samples = 0; sig_pos = false; pos = p_fall + 1; }
-                else { pos = p_open + 1; opened = true; break; }
-              } else {
-                const int p_rise = next_set128(GT_lo, GT_hi, pos);
-                if (p_rise >= nvalid) { n_samples += nvalid - pos; pos = nvalid; break; }
-                const int n_at = n_samples + (p_rise - pos + 1);
-                num_pulses = (n_at > half_pw) ? num_pulses + 1 : 0;
-                n_samples = 0; sig_pos = true; pos = p_rise + 1;
-              }
-            }
+            const int p_open = gate_closed_run<4>(ltw, gtw, run_start, nvalid, C.n_T1, half_pw, gs);
+            const bool opened = p_open >= 0;
+            pos = opened ? p_open + 1 : nvalid;
             // ---- DC tracker inputs for the closed run [run_start, pos) (gate_impl.cc:141-143); the run
             //      includes the trigger sample, as in the reference (the update precedes the open test)
             const int len = pos - run_start;
@@ -511,14 +398,12 @@ __global__ void __launch_bounds__(kFusedThreads, 8) rx_fused_kernel(const FusedA
                 ev.type = 1; ev.pos = pos - 1; ev.a = n_e - 1; ev.b = open_idx; ev.c = cur_store ? 1 : 0; ev.d = wcount & 1;
               }
               nev++;
-              num_pulses = 0;
-              n_samples = 1;
             }
           } else {
             // ---- open: the samples pass through (gate_impl.cc:182-195); emitted one tile later
-            const int take = min(to_ungate - n_samples, nvalid - pos);
-            n_samples += take; pos += take;
-            if (n_samples >= to_ungate) {
+            const int take = min(to_ungate - gs.n_samples, nvalid - pos);
+            gs.n_samples += take; pos += take;
+            if (gs.n_samples >= to_ungate) {
               gate_open = false;
               const int kind = wcount & 1;  // windows alternate RN16, EPC (SURVEY.md 3.5)
               if (lane == 0 && nev < kMaxTileEvents) {
@@ -531,7 +416,7 @@ __global__ void __launch_bounds__(kFusedThreads, 8) rx_fused_kernel(const FusedA
               // the Gen2 logic answers (ACK after RN16 -> GATE_SEEK_EPC, Query/QueryRep after EPC ->
               // GATE_SEEK_RN16) and the next gate call applies it (gate_impl.cc:112-123)
               to_ungate = kind ? C.len_rn16 : C.len_epc;
-              n_samples = 0;
+              gs.n_samples = 0;
               if (kind) {
                 nq++;
                 if (nq > C.max_queries) { terminated = true; break; }  // gate_impl.cc:101-109

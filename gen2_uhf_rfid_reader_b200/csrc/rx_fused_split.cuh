@@ -1,12 +1,12 @@
 // rx_fused_split.cuh -- fast-path variant of the fused capture kernel (reference configuration and every
-// rate whose amplitude / DC rings fit one tile, i.e. raw rates up to 5 MS/s).
+// rate whose amplitude / DC rings fit one tile, i.e. raw rates up to 2.56 MS/s).
 //
 // Same arithmetic as rx_fused.cuh, different schedule.  The order-dependent work of a segment is split over
 // TWO warps that run concurrently, one tile apart:
 //   chain    ONLY the three float running sums (lane 0: avg_ampl over tile i, gate_impl.cc:131; lanes 1,2:
 //            dc_est.re/.im over the closed samples of tile i-2, gate_impl.cc:141).  This is the irreducible
 //            serial part of exact replay: ~5.6 cycles per sample, nothing else on its critical path.
-//   control  thresholds (ballot into 128-bit masks), the edge/pulse state machine by bit-mask hopping, the few
+//   control  thresholds (ballot into 128-bit masks), the edge/pulse state machine (rx_gate.cuh), the few
 //            DC-ring differences that the workers could not pre-compute (tiles with gate activity), window
 //            emission to the L2-resident scratch two tiles later (when dc_est at the trigger is known), window
 //            hand-off to the decoder.
@@ -16,6 +16,7 @@
 #pragma once
 
 #include "rx_fused.cuh"
+#include "rx_gate.cuh"
 
 namespace rfid_b200 {
 
@@ -81,127 +82,6 @@ __device__ __forceinline__ void mbar_wait_lazy(uint64_t* bar, uint32_t parity)
 __device__ __forceinline__ void mbar_wait_hot(uint64_t* bar, uint32_t parity)
 {
   mbar_wait_relaxed(bar, parity, 2000);  // try_wait with a suspend hint: the hardware parks the warp until the phase flips
-}
-
-// ---- the edge/pulse state machine of one closed run, warp-parallel -------------------------------------
-// The reference walks the samples one by one (gate_impl.cc:145-180):
-//     n_samples++;  POS && a<thr -> NEG, n_samples=0;   NEG && a>thr -> POS, pulse bookkeeping, n_samples=0;
-//     open when n_samples > T1 && POS && num_pulses > 5.
-// Here: (1) the POS/NEG state before every position follows from the fall-wish / rise-wish masks by a carry
-// chain -- state' = rise | (keep & state) is the carry recurrence of a binary addition, so one 128-bit add gives
-// all 128 states; (2) the resulting edges (<= 32 per batch) are handled one per lane: pulse widths by a shuffle,
-// the run-length of consecutive valid pulses by ballot + popc, the first position at which the gate opens by
-// ballot + ffs.  Exactly the reference's decisions, O(1) warp steps per tile instead of one step per edge.
-struct GateFsm {
-  bool sig_pos;
-  int n_samples, num_pulses;
-};
-
-__device__ __forceinline__ int kth_set_bit128(unsigned w0, unsigned w1, unsigned w2, unsigned w3, int k)
-{
-  const int c0 = __popc(w0), c1 = c0 + __popc(w1), c2 = c1 + __popc(w2);
-  int word = 0, r = k;
-  unsigned sel = w0;
-  if (k >= c2) { word = 3; r = k - c2; sel = w3; }
-  else if (k >= c1) { word = 2; r = k - c1; sel = w2; }
-  else if (k >= c0) { word = 1; r = k - c0; sel = w1; }
-  return 32 * word + (int)__fns(sel, 0, r + 1);
-}
-
-// Processes the closed samples [from, nvalid) of a tile.  Returns the position at which the gate opens
-// (the trigger sample, state updated for the open gate) or -1 (state advanced to the end of the tile).
-struct Mask128 { unsigned w[4]; };
-
-__device__ __forceinline__ int fsm_closed_run(const Mask128& lt, const Mask128& gt, int from, int nvalid, int n_T1,
-                                              int half_pw, GateFsm& st)
-{
-  const int lane = threadIdx.x & 31;
-  // ---- states by carry propagation: A = rise|keep, B = rise, carry-in = current state
-  unsigned F[4], R[4], X[4];
-  unsigned carry = st.sig_pos ? 1u : 0u;
-#pragma unroll
-  for (int w = 0; w < 4; w++) {
-    // positions before `from` keep the state (they belong to an earlier run / an open window)
-    const int lo = from - 32 * w;
-    const unsigned live = lo <= 0 ? 0xffffffffu : (lo >= 32 ? 0u : (0xffffffffu << lo));
-    F[w] = lt.w[w] & live;
-    R[w] = gt.w[w] & live;
-    const unsigned Pk = ~(F[w] | R[w]);
-    const unsigned Aw = R[w] | Pk, Bw = R[w];
-    const unsigned long long sum = (unsigned long long)Aw + Bw + carry;
-    X[w] = Pk ^ (unsigned)sum;  // carry INTO each bit = state before that position (A ^ B == keep)
-    carry = (unsigned)(sum >> 32);
-  }
-  unsigned E[4], RS[4];
-#pragma unroll
-  for (int w = 0; w < 4; w++) {
-    RS[w] = ~X[w] & R[w];          // NEG -> POS
-    E[w] = (X[w] & F[w]) | RS[w];  // POS -> NEG, or rise
-  }
-  int pos = from;
-  int remaining = __popc(E[0]) + __popc(E[1]) + __popc(E[2]) + __popc(E[3]);
-  int done = 0;
-  while (true) {
-    const int nb = min(32, remaining);
-    // candidate before the first edge of this batch (the state may already be armed)
-    int first_edge = nvalid;
-    int p_k = 1 << 20;
-    bool is_rise = false;
-    if (lane < nb) {
-      p_k = kth_set_bit128(E[0], E[1], E[2], E[3], done + lane);
-      const int wsel = p_k >> 5;
-      const unsigned rsw = wsel == 0 ? RS[0] : (wsel == 1 ? RS[1] : (wsel == 2 ? RS[2] : RS[3]));
-      is_rise = (rsw >> (p_k & 31)) & 1u;
-    }
-    if (nb > 0) first_edge = __shfl_sync(0xffffffffu, p_k, 0);
-    if (st.sig_pos && st.num_pulses > kNumPulsesCommand) {
-      const int p_open = pos + max(0, n_T1 - st.n_samples);
-      if (p_open < first_edge && p_open < nvalid) {  // a falling edge at the same position wins
-        st.sig_pos = true; st.num_pulses = 0; st.n_samples = 1;
-        return p_open;
-      }
-    }
-    if (nb == 0) { st.n_samples += nvalid - pos; return -1; }
-    // ---- one edge per lane
-    const int p_virtual = pos - 1 - st.n_samples;  // where the previous edge would sit
-    int p_prev = __shfl_up_sync(0xffffffffu, p_k, 1);
-    if (lane == 0) p_prev = p_virtual;
-    const bool valid_rise = (lane < nb) && is_rise && (p_k - p_prev > half_pw);   // n_samples > n_samples_PW/2
-    const bool bad_rise = (lane < nb) && is_rise && !(p_k - p_prev > half_pw);
-    const unsigned VR = __ballot_sync(0xffffffffu, valid_rise), IR = __ballot_sync(0xffffffffu, bad_rise);
-    // num_pulses after edge k: valid rises since the last invalid one (inclusive range), plus the carried
-    // count if no reset happened yet
-    const unsigned upto = lane == 31 ? 0xffffffffu : ((2u << lane) - 1u);
-    const unsigned resets = IR & upto;
-    int np;
-    if (resets) {
-      const int last = 31 - __clz(resets);
-      np = __popc(VR & upto & ~((2u << last) - 1u));
-    } else {
-      np = st.num_pulses + __popc(VR & upto);
-    }
-    // next edge after lane k (next lane, or the first edge of the next batch, or none)
-    int p_next = __shfl_down_sync(0xffffffffu, p_k, 1);
-    if (lane == nb - 1) p_next = (remaining > nb) ? kth_set_bit128(E[0], E[1], E[2], E[3], done + nb) : nvalid;
-    const int p_open_k = p_k + 1 + n_T1;
-    const bool opens = (lane < nb) && is_rise && np > kNumPulsesCommand && p_open_k < p_next && p_open_k < nvalid;
-    const unsigned OM = __ballot_sync(0xffffffffu, opens);
-    if (OM) {
-      const int k = __ffs(OM) - 1;
-      const int p_open = __shfl_sync(0xffffffffu, p_open_k, k);
-      st.sig_pos = true; st.num_pulses = 0; st.n_samples = 1;
-      return p_open;
-    }
-    // ---- no opening in this batch: state after its last edge
-    const int kl = nb - 1;
-    const int p_last = __shfl_sync(0xffffffffu, p_k, kl);
-    st.sig_pos = __shfl_sync(0xffffffffu, (int)is_rise, kl) != 0;
-    st.num_pulses = __shfl_sync(0xffffffffu, np, kl);
-    st.n_samples = 0;
-    pos = p_last + 1;
-    done += nb;
-    remaining -= nb;
-  }
 }
 
 template <int DECIM, int MFQ>
@@ -277,29 +157,16 @@ __global__ void __launch_bounds__(kSplitThreads, 7) rx_fused_split_kernel(const 
   if (role >= 2 && role < 2 + kSWWarps) {
     // =========================================================== workers
     const int wt = (role - 2) * 32 + lane;
-    // raw tile geometry.  Tile k >= 1 starts at raw sample D*kTT*k - (D-1) of the segment, moved down to an even
-    // absolute index (16-byte TMA source); tile 0 starts at the segment's first (even-aligned) sample.  Interior
-    // tiles are all alike: `fast_tiles` of them can be issued with a constant byte count and a pointer bump.
+    // raw tile geometry (interior_tiles): tile k >= 1 starts at raw sample D*kTT*k - (D-1) - odd of the segment
     const int odd = (int)(sg.offset & 1ull);
-    const uint32_t fast_bytes = (uint32_t)((DECIM * kTT + 2 * odd) * 8);
-    int fast_tiles = 0;  // tiles 1 .. fast_tiles-1 take the fast path
-    {
-      // tile k is "interior" when its last sample D*(k*kTT + kTT-1) exists and the rounded-up copy stays inside the capture
-      const long long by_len = ((long long)sg.length - 1 - (long long)DECIM * (kTT - 1)) / ((long long)DECIM * kTT);
-      const long long room = (long long)A.n_raw - (long long)sg.offset + (DECIM - 1) + odd - (DECIM * kTT + 2 * odd);
-      const long long by_buf = room >= 0 ? room / ((long long)DECIM * kTT) : -1;
-      long long f = (by_len < by_buf ? by_len : by_buf) + 1;
-      if (sg.length < (unsigned)(DECIM * kTT)) f = 0;
-      fast_tiles = f < 0 ? 0 : (f > ntiles ? ntiles : (int)f);
-    }
-    const float2* const fast_src = A.iq + sg.offset - (DECIM - 1) - odd;  // + D*kTT*k for tile k >= 1
+    const InteriorTiles fast = interior_tiles<DECIM>(A.iq, A.n_raw, sg, ntiles);
     auto load_tile = [&](int k, int rs_) {
       float2* dst = raw + (size_t)rs_ * A.raw_stage_samples;
-      if (k >= 1 && k < fast_tiles) {
-        mbar_arrive_expect_tx(&B.raw_full[rs_], fast_bytes);
-        tma_load_1d(dst, fast_src + (size_t)k * (DECIM * kTT), fast_bytes, &B.raw_full[rs_]);
+      if (k >= 1 && k < fast.n) {
+        mbar_arrive_expect_tx(&B.raw_full[rs_], fast.bytes);
+        tma_load_1d(dst, fast.src + (size_t)k * (DECIM * kTT), fast.bytes, &B.raw_full[rs_]);
       } else {
-        issue_tile_load<DECIM>(A, sg, k, dst, &B.raw_full[rs_]);
+        issue_tile_load<DECIM>(A.iq, A.n_raw, sg, k, dst, &B.raw_full[rs_]);
       }
     };
     if (wt == 0) {
@@ -699,8 +566,7 @@ __global__ void __launch_bounds__(kSplitThreads, 7) rx_fused_split_kernel(const 
     PH_END(20)
   } else if (role == 1) {
     // =========================================================== control
-    bool sig_pos = false;          // signal_state, starts NEG_EDGE (gate_impl.cc:45)
-    int n_samples = 0, num_pulses = 0;
+    GateFsm gs = {false, 0, 0};    // signal_state starts NEG_EDGE (gate_impl.cc:45)
     bool gate_open = false;
     int to_ungate = C.len_rn16;    // first SEEK is for an RN16 (global_vars.cc:47, reader_impl.cc:262)
     int wcount = 0, open_idx = 0;
@@ -727,48 +593,17 @@ __global__ void __launch_bounds__(kSplitThreads, 7) rx_fused_split_kernel(const 
         float* er = etile + (s * 2 + 0) * kTT;
         float* ei = er + kTT;
         if (!terminated) {
-          // thresholds of tile i (gate_impl.cc:136,148,154): a < 0.75 avg / a > 0.75 avg per sample, as 128-bit masks.
-          // A tile that lies entirely inside an open window needs none (the gate ignores edges while it is open).
-          unsigned lt[4] = {0u, 0u, 0u, 0u}, gt[4] = {0u, 0u, 0u, 0u};
-          if (!(gate_open && to_ungate - n_samples > nvalid)) {
-#pragma unroll
-            for (int r = 0; r < 4; r++) {
-              const int p = r * 32 + lane;
-              const float thr = f_mul(davg[p], kThreshFraction);
-              const float a = ta[p];
-              lt[r] = __ballot_sync(0xffffffffu, a < thr);
-              gt[r] = __ballot_sync(0xffffffffu, a > thr);
-            }
-            if (nvalid < kTT) {  // the segment's last, partial tile: samples past its end compare nothing
-#pragma unroll
-              for (int r = 0; r < 4; r++) {
-                const int left = nvalid - r * 32;
-                const unsigned vm = left >= 32 ? 0xffffffffu : (left > 0 ? (1u << left) - 1u : 0u);
-                lt[r] &= vm;
-                gt[r] &= vm;
-              }
-            }
-          }
+          // thresholds of tile i, word (lane & 3) of the masks.  A tile that lies entirely inside an open window needs none
+          // (the gate ignores edges while it is open).
+          unsigned ltw = 0u, gtw = 0u;
+          if (!(gate_open && to_ungate - gs.n_samples > nvalid)) gate_masks<4>(davg, ta, nvalid, ltw, gtw);
           PH_MARK(2)
           int pos = 0;
           while (pos < nvalid) {
             if (!gate_open) {
               // ---- closed: edges, pulse counting and the open test of this run in one warp-parallel step
               const int run_start = pos;
-              int p_open = -1;
-              if (sig_pos && (lt[0] | lt[1] | lt[2] | lt[3]) == 0u) {
-                // carrier only (the common case): no falling edge can occur, only the open test remains
-                if (num_pulses > kNumPulsesCommand) {
-                  const int cand = run_start + max(0, C.n_T1 - n_samples);
-                  if (cand < nvalid) { p_open = cand; num_pulses = 0; n_samples = 1; }
-                }
-                if (p_open < 0) n_samples += nvalid - run_start;
-              } else {
-                GateFsm fs = {sig_pos, n_samples, num_pulses};
-                const Mask128 ltm = {{lt[0], lt[1], lt[2], lt[3]}}, gtm = {{gt[0], gt[1], gt[2], gt[3]}};
-                p_open = fsm_closed_run(ltm, gtm, run_start, nvalid, C.n_T1, half_pw, fs);
-                sig_pos = fs.sig_pos; n_samples = fs.n_samples; num_pulses = fs.num_pulses;
-              }
+              const int p_open = gate_closed_run<4>(ltw, gtw, run_start, nvalid, C.n_T1, half_pw, gs);
               const bool opened = p_open >= 0;
               pos = opened ? p_open + 1 : nvalid;
               // ---- DC tracker inputs of the closed run [run_start, pos) (gate_impl.cc:141-143; includes the trigger)
@@ -813,9 +648,9 @@ __global__ void __launch_bounds__(kSplitThreads, 7) rx_fused_split_kernel(const 
               }
             } else {
               // ---- open: samples pass through (gate_impl.cc:182-195); emitted two tiles later
-              const int take = min(to_ungate - n_samples, nvalid - pos);
-              n_samples += take; pos += take;
-              if (n_samples >= to_ungate) {
+              const int take = min(to_ungate - gs.n_samples, nvalid - pos);
+              gs.n_samples += take; pos += take;
+              if (gs.n_samples >= to_ungate) {
                 gate_open = false;
                 const int kind = wcount & 1;  // windows alternate RN16, EPC (SURVEY.md 3.5)
                 if (lane == 0 && nev < kMaxTileEvents) {
@@ -827,7 +662,7 @@ __global__ void __launch_bounds__(kSplitThreads, 7) rx_fused_split_kernel(const 
                 closed_since = 0;
                 // ACK after RN16 -> GATE_SEEK_EPC, Query/QueryRep after EPC -> GATE_SEEK_RN16 (gate_impl.cc:112-123)
                 to_ungate = kind ? C.len_rn16 : C.len_epc;
-                n_samples = 0;
+                gs.n_samples = 0;
                 if (kind) {
                   nq++;
                   if (nq > C.max_queries) { terminated = true; break; }  // gate_impl.cc:101-109

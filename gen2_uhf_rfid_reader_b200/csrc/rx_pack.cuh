@@ -1,5 +1,6 @@
 // rx_pack.cuh -- the roofline kernel of the reference configuration (decimation 5, 25 taps, rings inside one tile):
-// same arithmetic as rx_fused_split.cuh, re-scheduled around three measurements (tools/pack_profile.py, ncu):
+// same arithmetic as rx_fused_split.cuh (the gate of rx_gate.cuh, the raw-tile loader and running-sum replay of
+// rx_common.cuh, the decoder of rx_decode.cuh), re-scheduled around three measurements (tools/pack_profile.py, ncu):
 //   * the exact replay of the gate's float running sums (avg_ampl, gate_impl.cc:131; dc_est, gate_impl.cc:141) is a
 //     dependent FADD chain -- it costs the same whether 3 or 24 lanes of the warp carry a chain;
 //   * everything else of a segment is one warp's worth of *latency*, not of issue slots: a warp that walks a tile through
@@ -55,7 +56,8 @@
 //                      Its next instructions are the wait for tile t, against pas tiles of P1 of the other warps.
 #pragma once
 
-#include "rx_fused_split.cuh"
+#include "rx_decode.cuh"
+#include "rx_gate.cuh"
 
 namespace rfid_b200 {
 
@@ -154,120 +156,6 @@ struct PackCtaCtl {
 
 // hand-off waits on the critical path: the hardware parks the warp for a few dozen cycles per try
 __device__ __forceinline__ void pwait(uint64_t* bar, uint32_t parity) { mbar_wait_relaxed(bar, parity, 2000); }
-
-// ---- the edge / pulse state machine of one closed run on 256-bit masks, the eight mask words spread over lanes 0..7 ----
-// Same decisions as fsm_closed_run (rx_fused_split.cuh) and therefore as the reference's sample loop
-// (gate_impl.cc:145-180):
-//   states     state' = rise | keep & state is the carry recurrence of a binary addition; inside a word one 64-bit add,
-//              across the words the same recurrence once more (generate = the word's sum overflows with carry-in 0,
-//              propagate = only with carry-in 1), i.e. one more addition on the two ballots
-//   pulses     a rise at p is a valid pulse when the fall before it is more than half_pw back: no fall bit at p-1 .. p-half_pw
-//   num_pulses valid rises since the last invalid one (plus the carried count while no invalid rise has occurred)
-//   opening    the carried state reaches T1 before the first edge, or a rise r with num_pulses > 5 is followed by
-//              n_T1 + 1 edge-free samples inside the tile (gate opens at r + 1 + n_T1; a fall there wins)
-// Positions and counts are combined with redux.sync / vote (one instruction each); the reductions of the common path
-// (a tile full of reader pulses, no opening) do not depend on each other, so they are in flight together.
-struct GateFsm2 {
-  bool sig_pos;
-  int n_samples, num_pulses;
-};
-__device__ __forceinline__ unsigned m_below(int n) { return n <= 0 ? 0u : (n >= 32 ? 0xffffffffu : ((1u << n) - 1u)); }
-
-// ltw / gtw: word (lane & 7) of the below- / above-threshold masks, held by the lane itself
-__device__ __forceinline__ int fsm_closed_run_lanes(unsigned ltw, unsigned gtw, int from, int nvalid, int n_T1,
-                                                    int half_pw, GateFsm2& st)
-{
-  const unsigned FULL = 0xffffffffu;
-  const int lane = threadIdx.x & 31;
-  const int w = lane & 7;
-  const bool own = lane < 8;
-  const int base = 32 * w;
-  const unsigned live = own ? ~m_below(from - base) : 0u;   // (lanes 8..31 carry empty words)
-  const unsigned F = ltw & live, R = gtw & live;
-  const unsigned Pk = ~(F | R);
-  const unsigned long long sum0 = (unsigned long long)(R | Pk) + R, sum1 = sum0 + 1ull;
-  const unsigned C0 = __ballot_sync(FULL, own && (sum0 >> 32) != 0ull) & 0xffu;
-  const unsigned C1 = __ballot_sync(FULL, own && (sum1 >> 32) != 0ull) & 0xffu;
-  const unsigned cv = (C1 + C0 + (st.sig_pos ? 1u : 0u)) ^ C1 ^ C0;   // bit k: carry into word k (C0 is a subset of C1)
-  const unsigned X = Pk ^ (unsigned)(((cv >> w) & 1u) ? sum1 : sum0);   // state before each position
-  const unsigned RS = ~X & R, FE = X & F, E = RS | FE;
-  const int e_first = __reduce_min_sync(FULL, E ? base + __ffs(E) - 1 : 1024);
-  const int e_last = __reduce_max_sync(FULL, E ? base + 31 - __clz(E) : -1);
-  const int r_last = __reduce_max_sync(FULL, RS ? base + 31 - __clz(RS) : -1);
-  const unsigned fe_prev = __shfl_up_sync(FULL, FE, 1);
-  const int first_edge = e_first < nvalid ? e_first : nvalid;
-  if (st.sig_pos && st.num_pulses > kNumPulsesCommand) {
-    const int p_open = from + max(0, n_T1 - st.n_samples);
-    if (p_open < first_edge && p_open < nvalid) {
-      st.sig_pos = true; st.num_pulses = 0; st.n_samples = 1;
-      return p_open;
-    }
-  }
-  if (e_first >= nvalid) { st.n_samples += nvalid - from; return -1; }
-  const unsigned fe_lo = w == 0 ? 0u : fe_prev;
-  unsigned knock = 0u;
-  for (int k = 1; k <= half_pw; k++) knock |= (FE << k) | (fe_lo >> (32 - k));
-  unsigned VR = RS & ~knock;
-  // the first edge, if it is a rise: its pulse began before the run
-  if ((e_first >> 5) == w && ((RS >> (e_first & 31)) & 1u) && !(st.n_samples + (e_first - from + 1) > half_pw))
-    VR &= ~(1u << (e_first & 31));
-  const unsigned IR = RS & ~VR;
-  const int np_in = st.num_pulses;
-  const int lim = nvalid - 1 - n_T1;  // rises at or above lim cannot open the gate within this tile
-  // (host: n_T1 + 1 >= 32.)  A rise that opens the gate is followed by n_T1 + 1 edge-free positions; when that is 64 or
-  // more, the stretch covers a whole mask word, so a tile without an edge-free word below nvalid has no candidate.
-  if (lim > 0 && (n_T1 + 1 < 64 || __any_sync(FULL, own && base < nvalid && E == 0u))) {
-    auto first_of = [&](unsigned m) { return __reduce_min_sync(FULL, m ? base + __ffs(m) - 1 : 1024); };
-    auto last_of = [&](unsigned m) { return __reduce_max_sync(FULL, m ? base + 31 - __clz(m) : -1); };
-    auto np_at = [&](int r) {  // num_pulses right after the rise at r
-      const unsigned upto = m_below(r + 1 - base);
-      const int last = last_of(IR & upto);
-      const unsigned rng = upto & ~m_below(last + 1 - base);
-      const int cnt = __reduce_add_sync(FULL, __popc(VR & rng));
-      return last >= 0 ? cnt : np_in + cnt;
-    };
-    // inside its own word an opening rise is the highest edge; the first edge of the words above it (suffix minimum over
-    // the lanes) decides.  At most nvalid / (n_T1 + 1) rises qualify, so the loop below runs once or twice.
-    const int hi = E ? 31 - __clz(E) : -1;
-    const int fe = E ? base + __ffs(E) - 1 : 1024;
-    int nx = __shfl_down_sync(FULL, fe, 1);
-    if (w == 7) nx = 1024;
-    {
-      int t1 = __shfl_down_sync(FULL, nx, 1); if (w >= 6) t1 = 1024; nx = min(nx, t1);
-      int t2 = __shfl_down_sync(FULL, nx, 2); if (w >= 5) t2 = 1024; nx = min(nx, t2);
-      int t4 = __shfl_down_sync(FULL, nx, 4); if (w >= 3) t4 = 1024; nx = min(nx, t4);
-    }
-    const int rr = base + hi;
-    const bool q = own && hi >= 0 && ((RS >> hi) & 1u) && rr < lim && nx > rr + 1 + n_T1;
-    unsigned cand = q ? (1u << hi) : 0u;
-    while (true) {
-      const int r = first_of(cand);
-      if (r >= 1024) break;
-      if (own && (r >> 5) == w) cand &= ~(1u << (r & 31));
-      const unsigned quiet_rng = m_below(r + 2 + n_T1 - base) & ~m_below(r + 1 - base);
-      if (!__any_sync(FULL, (E & quiet_rng) != 0u) && np_at(r) > kNumPulsesCommand) {
-        st.sig_pos = true; st.num_pulses = 0; st.n_samples = 1;
-        return r + 1 + n_T1;
-      }
-    }
-  }
-  st.sig_pos = e_last == r_last;            // the last edge is a rise
-  st.n_samples = nvalid - 1 - e_last;
-  if (r_last >= 0) {
-    // valid rises after the last invalid one: the words above the last word that holds an invalid rise, and that word's
-    // bits above it
-    const unsigned Lm = __ballot_sync(FULL, IR != 0u) & 0xffu;
-    unsigned mine = VR;
-    if (Lm) {
-      const int L = 31 - __clz(Lm);
-      if (w < L) mine = 0u;
-      else if (w == L && IR) mine = VR & ~((2u << (31 - __clz(IR))) - 1u);
-    }
-    const int cnt = __reduce_add_sync(FULL, own ? __popc(mine) : 0);
-    st.num_pulses = Lm ? cnt : np_in + cnt;
-  }
-  return -1;
-}
 
 // One claimed phase of a window's decode (decoder pool): act 1 the head, 2 one chunk of the symbol-period search, 3 the
 // rest (the head if not yet run, the remaining chunks, bit decisions, CRC) and the record.  The decode's state comes
@@ -640,8 +528,7 @@ __global__ void __launch_bounds__(kPackMaxThreads, 1) rx_pack_kernel(const PackA
     } else {
       // ------------------------------------------------------------------------------------- warp B: P3
       // the gate (gate_impl.cc:45, global_vars.cc:47, reader_impl.cc:259,262)
-      bool sig_pos = false;
-      int n_samples = 0, num_pulses = 0;
+      GateFsm gs = {false, 0, 0};
       bool gate_open = false;
       int to_ungate = C.len_rn16;
       bool terminated = false;
@@ -678,17 +565,17 @@ __global__ void __launch_bounds__(kPackMaxThreads, 1) rx_pack_kernel(const PackA
           auto release_a = [&]() {   // this tile's |y| and avg_ampl have been read for the last time
             if (!freed) { __syncwarp(); if (lane == 0) mbar_arrive(&B.freeA[t % PAS]); freed = true; }
           };
-          if (!terminated && gate_open && to_ungate - n_samples > nvalid) {
+          if (!terminated && gate_open && to_ungate - gs.n_samples > nvalid) {
             // the whole tile lies inside an open window (gate_impl.cc:182-195): nothing to detect, no DC update
             release_a();
-            n_samples += nvalid;   // (n_e = 0: the chain warp skips the tile)
+            gs.n_samples += nvalid;   // (n_e = 0: the chain warp skips the tile)
           } else if (!terminated) {
             // thresholds (gate_impl.cc:136,148,154).  First a one-vote test in the lanes' natural 4-sample groups: while the
             // signal is high and no sample of the tile falls below its threshold, no edge can occur (carrier only).
-            unsigned ltw = 0u, gtw = 0u;   // word (lane & 7) of the below- / above-threshold masks
+            unsigned ltw = 0u, gtw = 0u;   // word (lane & 7) of the below- / above-threshold masks (gate_masks)
             // (only tried when the previous tile was edge-free too: inside a reader command the test would fail every time)
             bool quiet = false;
-            if (sig_pos && !gate_open && nvalid == kT2 && was_quiet) {
+            if (gs.sig_pos && !gate_open && nvalid == kT2 && was_quiet) {
               bool below = false;
 #pragma unroll
               for (int h2 = 0; h2 < 2; h2++) {
@@ -700,46 +587,20 @@ __global__ void __launch_bounds__(kPackMaxThreads, 1) rx_pack_kernel(const PackA
               quiet = !__any_sync(0xffffffffu, below);
             }
             bool have_masks = false;
-            auto make_masks = [&]() {
-#pragma unroll
-              for (int r = 0; r < 8; r++) {
-                const int p = r * 32 + lane;
-                const float thr = f_mul(davg[p], kThreshFraction);
-                const float av = ta[p];
-                const unsigned bl = __ballot_sync(0xffffffffu, av < thr), bg = __ballot_sync(0xffffffffu, av > thr);
-                if ((lane & 7) == r) { ltw = bl; gtw = bg; }
-              }
-              if (nvalid < kT2) {
-                const unsigned vm = m_below(nvalid - (lane & 7) * 32);
-                ltw &= vm;
-                gtw &= vm;
-              }
-              have_masks = true;
-              release_a();
-            };
             int pos = 0;
             while (pos < nvalid) {
               if (!gate_open) {
                 const int run_start = pos;
-                int p_open = -1;
                 // (the one-vote result only covers a run that starts the tile with the signal high)
                 PP_AT(4)
-                if (!have_masks && !(quiet && run_start == 0)) make_masks();
-                PP_AT(5)
-                const bool no_lt = !__any_sync(0xffffffffu, ltw != 0u);
-                was_quiet = no_lt;
-                if (sig_pos && no_lt) {
-                  // carrier only (the common case): no falling edge can occur, only the open test remains
-                  if (num_pulses > kNumPulsesCommand) {
-                    const int cand = run_start + max(0, C.n_T1 - n_samples);
-                    if (cand < nvalid) { p_open = cand; num_pulses = 0; n_samples = 1; }
-                  }
-                  if (p_open < 0) n_samples += nvalid - run_start;
-                } else {
-                  GateFsm2 fs = {sig_pos, n_samples, num_pulses};
-                  p_open = fsm_closed_run_lanes(ltw, gtw, run_start, nvalid, C.n_T1, C.n_PW / 2, fs);
-                  sig_pos = fs.sig_pos; n_samples = fs.n_samples; num_pulses = fs.num_pulses;
+                if (!have_masks && !(quiet && run_start == 0)) {
+                  gate_masks<8>(davg, ta, nvalid, ltw, gtw);
+                  have_masks = true;
+                  release_a();
                 }
+                PP_AT(5)
+                was_quiet = !__any_sync(0xffffffffu, ltw != 0u);
+                const int p_open = gate_closed_run<8>(ltw, gtw, run_start, nvalid, C.n_T1, C.n_PW / 2, gs);
                 PP_AT(6)
                 const bool opened = p_open >= 0;
                 pos = opened ? p_open + 1 : nvalid;
@@ -807,11 +668,11 @@ __global__ void __launch_bounds__(kPackMaxThreads, 1) rx_pack_kernel(const PackA
               } else {
                 // ---- open: samples pass through (gate_impl.cc:182-195); warp C reads them from the history.  They do not
                 // enter the DC tracker: their list entries carry the running sums unchanged
-                const int take = min(to_ungate - n_samples, nvalid - pos);
+                const int take = min(to_ungate - gs.n_samples, nvalid - pos);
                 for (int j = lane; j < take; j += 32) { er[pos + j] = -0.0f; ei[pos + j] = -0.0f; }
-                n_samples += take; pos += take;
+                gs.n_samples += take; pos += take;
                 n_e = pos;
-                if (n_samples >= to_ungate) {
+                if (gs.n_samples >= to_ungate) {
                   gate_open = false;
 #ifdef RFID_B200_PHASE_PROFILE
                   if (pp_cta && lane == 0) { unsigned long long tg; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(tg)); atomicMax(pp_cta + 2, tg); }
@@ -827,7 +688,7 @@ __global__ void __launch_bounds__(kPackMaxThreads, 1) rx_pack_kernel(const PackA
                   closed_since = 0;
                   // ACK after RN16 -> GATE_SEEK_EPC, Query/QueryRep after EPC -> GATE_SEEK_RN16 (gate_impl.cc:112-123)
                   to_ungate = kind ? C.len_rn16 : C.len_epc;
-                  n_samples = 0;
+                  gs.n_samples = 0;
                   if (kind && nq + 1 > C.max_queries) { terminated = true; break; }  // gate_impl.cc:101-109
                 }
               }
@@ -934,30 +795,16 @@ __global__ void __launch_bounds__(kPackMaxThreads, 1) rx_pack_kernel(const PackA
     const int nhalf = g < g_act ? (n_out + kTT - 1) / kTT : 0;
     PackSegCtl& B = ctl_all[g < G ? g : 0];
     float2* raw = reinterpret_cast<float2*>(smem + A.off_seg + (size_t)(g < G ? g : 0) * A.seg_bytes + A.o_raw);
-    // raw half-tile geometry (as rx_fused_split.cuh)
-    const int odd = (int)(sg.offset & 1ull);
-    const uint32_t fast_bytes = (uint32_t)((DECIM * kTT + 2 * odd) * 8);
-    int fast_tiles = 0;
-    {
-      const long long by_len = ((long long)sg.length - 1 - (long long)DECIM * (kTT - 1)) / ((long long)DECIM * kTT);
-      const long long room = (long long)A.n_raw - (long long)sg.offset + (DECIM - 1) + odd - (DECIM * kTT + 2 * odd);
-      const long long by_buf = room >= 0 ? room / ((long long)DECIM * kTT) : -1;
-      long long f = (by_len < by_buf ? by_len : by_buf) + 1;
-      if (sg.length < (unsigned)(DECIM * kTT)) f = 0;
-      fast_tiles = f < 0 ? 0 : (f > nhalf ? nhalf : (int)f);
-    }
-    const float2* const fast_src = A.iq + sg.offset - (DECIM - 1) - odd;
-    FusedArgs FA;  // issue_tile_load only reads iq / n_raw
-    FA.iq = A.iq; FA.n_raw = A.n_raw;
+    const InteriorTiles fast = interior_tiles<DECIM>(A.iq, A.n_raw, sg, nhalf);
     const unsigned long long pol = l2_policy_evict_first();   // every raw sample is read exactly once
     auto issue = [&](int k) {
       const int rs_ = k & 1;
       float2* dst = raw + (size_t)rs_ * A.raw_stage_samples;
-      if (k >= 1 && k < fast_tiles) {
-        mbar_arrive_expect_tx(&B.raw_full[rs_], fast_bytes);
-        tma_load_1d_hint(dst, fast_src + (size_t)k * (DECIM * kTT), fast_bytes, &B.raw_full[rs_], pol);
+      if (k >= 1 && k < fast.n) {
+        mbar_arrive_expect_tx(&B.raw_full[rs_], fast.bytes);
+        tma_load_1d_hint(dst, fast.src + (size_t)k * (DECIM * kTT), fast.bytes, &B.raw_full[rs_], pol);
       } else {
-        issue_tile_load<DECIM>(FA, sg, k, dst, &B.raw_full[rs_]);
+        issue_tile_load<DECIM>(A.iq, A.n_raw, sg, k, dst, &B.raw_full[rs_]);
       }
     };
     for (int k = 0; k < 2 && k < nhalf; k++) issue(k);   // both stages are free at the start

@@ -134,16 +134,21 @@ def reference_outputs(iq):
 
 
 # (adc rate, taps) of the comparisons at other sample rates, one or more per kernel the library picks there:
+# rx_fused_split_kernel<5,5> at 0.4 and 0.6 MS/s (n_T1 + 1 < 32: a gate opening fits inside one 32-sample mask word),
 # rx_fused_split_kernel<5,0> / <5,5> at 1.0 MS/s, rx_pack_kernel at 1.2 MS/s, rx_fused_split_kernel<5,5> at 1.4-2.4 MS/s,
 # rx_fused_kernel from 2.6 MS/s up.  Every one is a well-defined rate (tests/rate_rule.py).
-RATES = [(1000000, 12), (1000000, 25), (1200000, 25), (1400000, 25), (1800000, 25), (2200000, 25), (2400000, 25),
-         (2600000, 25), (3000000, 25), (5000000, 25), (4000000, 50), (8000000, 100)]
+RATES = [(400000, 25), (600000, 25), (1000000, 12), (1000000, 25), (1200000, 25), (1400000, 25), (1800000, 25),
+         (2200000, 25), (2400000, 25), (2600000, 25), (3000000, 25), (5000000, 25), (4000000, 50), (8000000, 100)]
 # capture variants: name -> make_capture keywords ("quiet": noise- and drift-free, which makes exact ties for the
 # decoder's first-maximum rules)
 RATE_VARIANTS = {"default": dict(), "quiet": dict(noise_sigma=0.0, clock_ppm_pct=0.0), "notag": dict(n_tags=0),
                  "noisy": dict(noise_sigma=0.02)}
 RATE_Q4 = dict(fixed_q=4, n_tags=8)      # through the FIXED_Q = 4 build, at these rates only
 RATE_Q4_RATES = (1200000, 2400000)
+# heavy noise, at these rates only: rx_fused_kernel's rates have half_pw >= 3, where only noise dips of exactly half_pw
+# samples test the gate's pulse-width rule at its boundary
+RATE_GLITCH = dict(noise_sigma=0.2)
+RATE_GLITCH_RATES = (2600000, 4000000)
 
 
 def rate_cases():
@@ -154,6 +159,8 @@ def rate_cases():
             out.append(("r%d_t%d_%s" % (adc, ntaps, name), adc, ntaps, kw))
         if adc in RATE_Q4_RATES:
             out.append(("r%d_t%d_q4" % (adc, ntaps), adc, ntaps, RATE_Q4))
+        if adc in RATE_GLITCH_RATES:
+            out.append(("r%d_t%d_glitch" % (adc, ntaps), adc, ntaps, RATE_GLITCH))
     return out
 
 

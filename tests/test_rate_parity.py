@@ -1,9 +1,9 @@
 """GPU tests at sample rates other than 2 MS/s (run with -m gpu on an H100).
 
 Every kernel the library picks is compared, bit for bit, with the reference's own blocks (stored outputs in
-tests/golden/reference_rates.npz) and with the C restatement, at one or more rates per kernel: rx_fused_split_kernel<5,0>
-and <5,5> at 1.0 MS/s, rx_pack_kernel at 1.2 MS/s (25 taps), rx_fused_split_kernel<5,5> at 1.4 - 2.4 MS/s, rx_fused_kernel
-from 2.6 MS/s up.  At 1.2 MS/s the packed kernel runs code the 2 MS/s configuration never reaches: n_T1 + 1 < 64 in the
+tests/golden/reference_rates.npz) and with the C restatement, at one or more rates per kernel: rx_fused_split_kernel<5,5>
+at 0.4 and 0.6 MS/s (n_T1 + 1 < 32, the gate's short-quiet branch), rx_fused_split_kernel<5,0> and <5,5> at 1.0 MS/s,
+rx_pack_kernel at 1.2 MS/s (25 taps), rx_fused_split_kernel<5,5> at 1.4 - 2.4 MS/s, rx_fused_kernel from 2.6 MS/s up.  At 1.2 MS/s the packed kernel runs code the 2 MS/s configuration never reaches: n_T1 + 1 < 64 in the
 closed-run scan, a DC divisor (28) without the verified fast division, and a DC lookback of 7 lanes instead of 12.
 """
 import os
