@@ -15,6 +15,8 @@
                             reference_outputs()), so that the suite runs where the reference is absent
   reference_rates.npz       oracle/_ref records and counts at other sample rates (rate_outputs(); regenerate it
                             alone with `make_golden.py rates`)
+  reference_pulses.npz      oracle/_ref records and counts on the pulse-train captures (pulse_outputs(); regenerate it
+                            alone with `make_golden.py pulses`)
 """
 import json
 import lzma
@@ -91,6 +93,7 @@ def main():
                   open(os.path.join(HERE, tag + "_ref_stats.json"), "w"), indent=1)
     reference_outputs(iq)
     rate_outputs()
+    pulse_outputs()
     print("golden regenerated:", sorted(os.listdir(HERE)))
 
 
@@ -181,8 +184,71 @@ def rate_outputs():
     np.savez_compressed(os.path.join(HERE, "reference_rates.npz"), **out)
 
 
+# Pulse-train captures (tests/test_gate_fsm.py): reader-like commands whose raw pulse widths, depths and quiet gaps are
+# swept finely around n_PW and n_T1, so that after the boxcar the decimated pulse widths and gaps straddle the gate's
+# bounds n_PW / 2 and n_T1.  One (adc rate, taps) per capture kernel configuration that decodes them.
+PULSE_RATES = [(400000, 25), (1000000, 25), (1200000, 25), (2000000, 25), (2400000, 25), (2600000, 25),
+               (4000000, 50), (8000000, 100)]
+PULSE_MAX_WINDOWS = 8
+
+
+def pulse_capture(adc, ntaps, n_segments=16, n_commands=8, decim=5):
+    """raw I/Q (complex64 ndarray) and segments: per segment a carrier lead-in, then n_commands times: 6-8 low pulses
+    (raw widths and depths swept around n_PW), a quiet gap swept around n_T1, one more pulse that ends the gap, and a
+    stretch of carrier (the window) that sometimes ends before the window does"""
+    from gen2_uhf_rfid_reader_b200 import abi
+    from oracle.pyoracle import derive_cfg
+    c = derive_cfg(adc_rate=adc, decim=decim, ntaps=ntaps)
+    hp, t1 = c.n_PW // 2, c.n_T1
+    rng = np.random.default_rng(adc // 1000 + ntaps)
+    parts, offs, lens, off = [], [], [], 0
+    for s in range(n_segments):
+        amp = 0.8 * np.exp(1j * rng.uniform(0, 2 * np.pi))
+        lvl = [np.ones(c.win_length * decim)]            # carrier lead-in: one avg_ampl window
+        for k in range(n_commands):
+            depth = rng.choice([0.0, 0.2, 0.4, 0.55])
+
+            def pulse(sweep):
+                # swept around n_PW / 2 after the boxcar, or clearly wider (a valid pulse)
+                lo, hi = ((max(1, (hp - 3) * decim), (hp + 4) * decim + ntaps) if sweep else
+                          ((hp + 2) * decim + ntaps // 2, (hp + 4) * decim + ntaps))
+                lvl.append(np.full(rng.integers(lo, hi + 1), depth))
+
+            for i in range(rng.integers(6, 9)):
+                pulse(rng.random() < 0.3)
+                lvl.append(np.ones(rng.integers(max(1, hp * decim), (3 * hp + 2) * decim + ntaps + 1)))
+            lo, hi = (t1 - 1) * decim - ntaps // 2, (t1 + 2) * decim + ntaps // 2
+            if rng.random() < 0.3:
+                lo, hi = lo - 2 * decim - ntaps // 2, hi + 2 * decim + ntaps // 2
+            lvl[-1] = np.ones(rng.integers(lo, hi + 1))   # the quiet gap
+            pulse(False)
+            lvl.append(np.ones(rng.integers(c.len_rn16, c.len_epc + 200) * decim))
+        x = np.concatenate(lvl) * amp
+        x = x + (rng.standard_normal(x.size) + 1j * rng.standard_normal(x.size)) * 0.004
+        parts.append(x.astype(np.complex64))
+        offs.append(off)
+        lens.append(x.size)
+        off += x.size
+    return np.concatenate(parts), abi.make_segments(offs, lens)
+
+
+def pulse_outputs():
+    """oracle/_ref on the pulse-train capture of each PULSE_RATES entry -> reference_pulses.npz"""
+    from oracle.refflow import RefFlow
+    ref = RefFlow(0)
+    out = {}
+    for adc, ntaps in PULSE_RATES:
+        iq, segs = pulse_capture(adc, ntaps)
+        key = "p%d_t%d" % (adc, ntaps)
+        out[key + "_records"], out[key + "_counts"], _ = ref.run_segments(iq, segs, adc_rate=adc, ntaps=ntaps,
+                                                                          max_per_seg=PULSE_MAX_WINDOWS)
+    np.savez_compressed(os.path.join(HERE, "reference_pulses.npz"), **out)
+
+
 if __name__ == "__main__":
     if sys.argv[1:] == ["rates"]:
         rate_outputs()
+    elif sys.argv[1:] == ["pulses"]:
+        pulse_outputs()
     else:
         main()
