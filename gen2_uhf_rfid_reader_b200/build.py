@@ -39,5 +39,25 @@ def build_library(force=False, verbose=False):
     return LIB
 
 
+def build_harness(src, lib, force=False):
+    """Compile a CUDA test harness (tests/cuda/*.cu) that includes csrc headers, with the library's flags; returns lib.
+    Rebuilds when stale or forced and nvcc exists; raises when there is neither nvcc nor a harness."""
+    if not force and os.path.exists(lib):
+        t = os.path.getmtime(lib)
+        if all(os.path.getmtime(d) <= t for d in [src] + glob.glob(os.path.join(CSRC, "*.cuh"))):
+            return lib
+    nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
+    if not os.path.exists(nvcc):
+        if os.path.exists(lib):
+            return lib
+        raise RuntimeError("nvcc not found and %s is missing" % lib)
+    subprocess.check_call([nvcc] + NVCC_FLAGS + ["-I", CSRC, "-o", lib, src], cwd=os.path.dirname(src))
+    return lib
+
+
+SC16_HARNESS_SRC = os.path.join(os.path.dirname(HERE), "tests", "cuda", "sc16_harness.cu")
+SC16_HARNESS = os.path.join(HERE, "libsc16_harness.so")
+
+
 if __name__ == "__main__":
     print(build_library(force=True, verbose=True))

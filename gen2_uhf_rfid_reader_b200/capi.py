@@ -14,6 +14,11 @@ from .build import LIB, build_library
 
 _lib = None
 
+# Default int16 -> float factor of sc16 captures: 1/32767, the factor UHD's host converters conventionally apply when they
+# widen the radio's sc16 samples to fc32 (full scale +-32767 -> +-1.0).  Decoding never depends on the value: an sc16
+# capture decodes, bit for bit, like its fc32 conversion np.float32(i) * np.float32(scale) with the same float.
+SC16_SCALE = float(np.float32(1.0 / 32767.0))
+
 
 class RfidB200Error(RuntimeError):
     pass
@@ -54,6 +59,8 @@ def load_library():
     L.rfid_b200_fs_dec.argtypes = [vp]
     L.rfid_b200_decode_capture.restype = C.c_int
     L.rfid_b200_decode_capture.argtypes = [vp, vp, C.c_size_t, vp, C.c_int, C.c_int, vp, vp, vp]
+    L.rfid_b200_decode_capture_sc16.restype = C.c_int
+    L.rfid_b200_decode_capture_sc16.argtypes = [vp, vp, C.c_size_t, C.c_float, vp, C.c_int, C.c_int, vp, vp, vp]
     L.rfid_b200_decode_capture_host.restype = C.c_int
     L.rfid_b200_decode_capture_host.argtypes = [vp, vp, C.c_size_t, vp, C.c_int, C.c_int, vp, vp]
     L.rfid_b200_last_launch_count.restype = C.c_int
@@ -75,6 +82,12 @@ def load_library():
     L.rfid_b200_default_segmenter.argtypes = [C.POINTER(abi.Segmenter)]
     L.rfid_b200_segment_capture.restype = C.c_int
     L.rfid_b200_segment_capture.argtypes = [vp, vp, C.c_size_t, C.POINTER(abi.Segmenter), vp, C.c_int, ip, vp]
+    L.rfid_b200_segment_capture_sc16.restype = C.c_int
+    L.rfid_b200_segment_capture_sc16.argtypes = [vp, vp, C.c_size_t, C.c_float, C.POINTER(abi.Segmenter), vp, C.c_int, ip,
+                                                 vp]
+    L.rfid_b200_ingest_capture_host_sc16.restype = C.c_int
+    L.rfid_b200_ingest_capture_host_sc16.argtypes = [vp, vp, C.c_size_t, C.c_float, C.POINTER(abi.Segmenter), C.c_int, vp,
+                                                     C.c_int, ip, vp, vp]
     L.rfid_b200_ingest_capture_host.restype = C.c_int
     L.rfid_b200_ingest_capture_host.argtypes = [vp, vp, C.c_size_t, C.POINTER(abi.Segmenter), C.c_int, vp, C.c_int, ip,
                                                 vp, vp]
@@ -97,7 +110,17 @@ EXPORTED_SYMBOLS = [
     "rfid_b200_reduce_stats", "rfid_b200_gate_work", "rfid_b200_decoder_work", "rfid_b200_mf_work",
     "rfid_b200_default_segmenter", "rfid_b200_segment_capture", "rfid_b200_ingest_capture_host",
     "rfid_b200_tx_synth", "rfid_b200_default_sim", "rfid_b200_sim_segment_length", "rfid_b200_sim_capture",
+    "rfid_b200_decode_capture_sc16", "rfid_b200_segment_capture_sc16", "rfid_b200_ingest_capture_host_sc16",
 ]
+
+
+def _sc16_samples(iq):
+    """complex samples of an int16 capture shaped (2n,) or (n, 2) (interleaved I, Q: UHD's sc16)"""
+    if iq.dim() == 2 and iq.shape[1] != 2 or iq.dim() > 2 or iq.numel() % 2:
+        raise ValueError("an int16 capture is shaped (2n,) or (n, 2): interleaved I, Q")
+    if not iq.is_contiguous():
+        raise ValueError("an int16 capture must be contiguous")
+    return iq.numel() // 2
 
 
 def default_sim(**kw):
@@ -161,18 +184,25 @@ class Gen2Rx:
                                                  self.lib.rfid_b200_last_cuda_error(self.h).decode()))
 
     # ---------------------------------------------------------------- capture mode
-    def decode_capture(self, iq, segs, max_windows=4, results=None, counts=None, stream=None):
-        """iq: CUDA complex64 (or float32 interleaved) tensor; segs: CUDA uint8/int64 tensor holding
-        rfid_b200_segment[nseg] (see `segments_to_device`).  Asynchronous on `stream` (default: the
-        current torch stream).  Returns (results uint8[nseg*max_windows,64], counts int32[nseg])."""
+    def decode_capture(self, iq, segs, max_windows=4, results=None, counts=None, stream=None, scale=SC16_SCALE):
+        """iq: CUDA complex64 (or float32 interleaved) tensor, or a torch.int16 tensor shaped (2n,) or (n, 2) holding an
+        sc16 capture (interleaved int16 I, Q), decoded as its conversion I * scale, Q * scale (`SC16_SCALE` by default);
+        segs: CUDA uint8/int64 tensor holding rfid_b200_segment[nseg] (see `segments_to_device`).  Asynchronous on
+        `stream` (default: the current torch stream).  Returns (results uint8[nseg*max_windows,64], counts int32[nseg])."""
         import torch
         nseg = segs.numel() * segs.element_size() // 16
-        n_raw = iq.numel() if iq.is_complex() else iq.numel() // 2
+        sc16 = iq.dtype == torch.int16
+        n_raw = _sc16_samples(iq) if sc16 else (iq.numel() if iq.is_complex() else iq.numel() // 2)
         if results is None:
             results = torch.zeros((nseg * max_windows, 64), dtype=torch.uint8, device=iq.device)
         if counts is None:
             counts = torch.zeros(nseg, dtype=torch.int32, device=iq.device)
         s = stream if stream is not None else torch.cuda.current_stream(iq.device)
+        if sc16:
+            rc = self.lib.rfid_b200_decode_capture_sc16(self.h, iq.data_ptr(), n_raw, scale, segs.data_ptr(), nseg,
+                                                        max_windows, results.data_ptr(), counts.data_ptr(), s.cuda_stream)
+            self._ck(rc, "rfid_b200_decode_capture_sc16")
+            return results, counts
         rc = self.lib.rfid_b200_decode_capture(self.h, iq.data_ptr(), n_raw, segs.data_ptr(), nseg, max_windows,
                                                results.data_ptr(), counts.data_ptr(), s.cuda_stream)
         self._ck(rc, "rfid_b200_decode_capture")
@@ -196,32 +226,51 @@ class Gen2Rx:
         self._ck(rc, "rfid_b200_decode_capture_host")
 
     # ---------------------------------------------------------------- capture ingest
-    def segment_capture(self, iq, segmenter=None, capacity=None, stream=None):
-        """CW-gap segment table (SEGMENT_DTYPE ndarray) of a CUDA capture tensor."""
+    def segment_capture(self, iq, segmenter=None, capacity=None, stream=None, scale=SC16_SCALE):
+        """CW-gap segment table (SEGMENT_DTYPE ndarray) of a CUDA capture tensor (complex64 / float32 interleaved, or an
+        sc16 torch.int16 tensor as in `decode_capture`, whose table is that of its conversion)."""
         import torch
-        n_raw = iq.numel() if iq.is_complex() else iq.numel() // 2
+        sc16 = iq.dtype == torch.int16
+        n_raw = _sc16_samples(iq) if sc16 else (iq.numel() if iq.is_complex() else iq.numel() // 2)
         cap = int(capacity) if capacity is not None else max(16, n_raw // 4096)
         segs = np.zeros(cap, dtype=abi.SEGMENT_DTYPE)
         n = C.c_int(0)
         s = stream if stream is not None else torch.cuda.current_stream(iq.device)
-        rc = self.lib.rfid_b200_segment_capture(self.h, iq.data_ptr(), n_raw, C.byref(segmenter) if segmenter else None,
-                                                segs.ctypes.data, cap, C.byref(n), s.cuda_stream)
-        self._ck(rc, "rfid_b200_segment_capture")
+        sp = C.byref(segmenter) if segmenter else None
+        if sc16:
+            rc = self.lib.rfid_b200_segment_capture_sc16(self.h, iq.data_ptr(), n_raw, scale, sp, segs.ctypes.data, cap,
+                                                         C.byref(n), s.cuda_stream)
+            self._ck(rc, "rfid_b200_segment_capture_sc16")
+        else:
+            rc = self.lib.rfid_b200_segment_capture(self.h, iq.data_ptr(), n_raw, sp, segs.ctypes.data, cap, C.byref(n),
+                                                    s.cuda_stream)
+            self._ck(rc, "rfid_b200_segment_capture")
         return segs[:n.value].copy()
 
-    def ingest_capture_host(self, iq, segmenter=None, max_windows=4, capacity=None):
-        """Recorded capture (host complex64 ndarray, e.g. np.fromfile/np.memmap) -> (segs, records, counts)."""
-        raw = np.ascontiguousarray(iq).view(np.float32).ravel()
+    def ingest_capture_host(self, iq, segmenter=None, max_windows=4, capacity=None, scale=SC16_SCALE):
+        """Recorded capture -> (segs, records, counts).  iq: host complex64 ndarray (e.g. np.fromfile / np.memmap of an
+        fc32 file), or an np.int16 array of interleaved I, Q (an sc16 file, e.g. np.memmap(path, dtype=np.int16)),
+        decoded as its conversion I * scale, Q * scale."""
+        sc16 = np.asarray(iq).dtype == np.int16
+        raw = np.ascontiguousarray(iq).ravel() if sc16 else np.ascontiguousarray(iq).view(np.float32).ravel()
+        if raw.size % 2:
+            raise ValueError("an interleaved I, Q capture has an even number of values")
         n_raw = raw.size // 2
         cap = int(capacity) if capacity is not None else max(16, n_raw // 4096)
         segs = np.zeros(cap, dtype=abi.SEGMENT_DTYPE)
         recs = np.zeros((cap, max_windows), dtype=abi.RESULT_DTYPE)
         counts = np.zeros(cap, dtype=np.int32)
         n = C.c_int(0)
-        rc = self.lib.rfid_b200_ingest_capture_host(self.h, raw.ctypes.data, n_raw, C.byref(segmenter) if segmenter else None,
-                                                    max_windows, segs.ctypes.data, cap, C.byref(n), recs.ctypes.data,
-                                                    counts.ctypes.data)
-        self._ck(rc, "rfid_b200_ingest_capture_host")
+        sp = C.byref(segmenter) if segmenter else None
+        if sc16:
+            rc = self.lib.rfid_b200_ingest_capture_host_sc16(self.h, raw.ctypes.data, n_raw, scale, sp, max_windows,
+                                                             segs.ctypes.data, cap, C.byref(n), recs.ctypes.data,
+                                                             counts.ctypes.data)
+            self._ck(rc, "rfid_b200_ingest_capture_host_sc16")
+        else:
+            rc = self.lib.rfid_b200_ingest_capture_host(self.h, raw.ctypes.data, n_raw, sp, max_windows, segs.ctypes.data,
+                                                        cap, C.byref(n), recs.ctypes.data, counts.ctypes.data)
+            self._ck(rc, "rfid_b200_ingest_capture_host")
         k = n.value
         return segs[:k].copy(), recs[:k].copy(), counts[:k].copy()
 

@@ -31,7 +31,8 @@ struct rfid_b200_ctx {
   cudaEvent_t ev_slice[4];
   std::string last_error;
   // capture mode
-  FusedArgs layout;     // shared-memory carve-up (pointers filled per call)
+  FusedArgs layout;     // shared-memory carve-up (pointers filled per call), fc32 captures
+  FusedArgs layout_sc16;  // the same for sc16 captures (raw stages of 4-byte samples)
   float* window_tap;
   int last_launches;
   bool timing;
@@ -188,11 +189,15 @@ int chunk_stage_samples(const RxConfig& c)
 // chunks and the rest of its RN16 windows gather from L2.
 
 // shared-memory carve-up of rx_fused_split_kernel: five tile stages forming one time-indexed ring
-void make_layout_split(const RxConfig& c, FusedArgs& L)
+// Raw stages hold a tile's samples in the capture's format (raw_bytes per sample, 8 fc32 or 4 sc16) plus the alignment of
+// its 16-byte granule (rx_common.cuh: issue_tile_load) and, for sc16, the read-ahead of the vector loads (sc16_run).
+int raw_stage_samples(const RxConfig& c, int raw_bytes) { return c.decim * kTT + (raw_bytes == 8 ? 2 : kSc16StagePad); }
+
+void make_layout_split(const RxConfig& c, int raw_bytes, FusedArgs& L)
 {
   int off = 0;
-  L.raw_stage_samples = c.decim * kTT + 2;
-  L.off_raw = off; off = align_up(off + kRawStages * L.raw_stage_samples * 8, 16);
+  L.raw_stage_samples = raw_stage_samples(c, raw_bytes);
+  L.off_raw = off; off = align_up(off + kRawStages * L.raw_stage_samples * raw_bytes, 16);
   L.bhist_size = next_pow2(kTT + c.mf_q + 2);
   L.off_bhist = off; off = align_up(off + L.bhist_size * 8 * (c.mf_rem ? 2 : 1), 16);
   L.off_tile_y = off; off += kRing * 8;
@@ -209,13 +214,13 @@ void make_layout_split(const RxConfig& c, FusedArgs& L)
   L.smem_bytes = off;
 }
 
-void make_layout(const RxConfig& c, FusedArgs& L)
+void make_layout(const RxConfig& c, int raw_bytes, FusedArgs& L)
 {
-  if (fast_path_ok(c)) { make_layout_split(c, L); return; }
+  if (fast_path_ok(c)) { make_layout_split(c, raw_bytes, L); return; }
   const bool spec = false;
   int off = 0;
-  L.raw_stage_samples = c.decim * kTT + 2;
-  L.off_raw = off; off = align_up(off + kRawStages * L.raw_stage_samples * 8, 16);
+  L.raw_stage_samples = raw_stage_samples(c, raw_bytes);
+  L.off_raw = off; off = align_up(off + kRawStages * L.raw_stage_samples * raw_bytes, 16);
   L.bhist_size = next_pow2(kTT + c.mf_q + 2);
   L.off_bhist = off; off = align_up(off + L.bhist_size * 8 * (c.mf_rem ? 2 : 1), 16);
   L.off_tile_y = off; off += kTileStages * kTT * 8;
@@ -258,18 +263,19 @@ bool pack_ok(const RxConfig& c)
 }
 
 // shared-memory carve-up of rx_pack_kernel for G segments per CTA
-void make_layout_pack(const RxConfig& c, int G, PackArgs& L)
+void make_layout_pack(const RxConfig& c, int G, int raw_bytes, PackArgs& L)
 {
   L.G = G;
   L.pas = pack_ring_slots(G);
   L.pds = L.pas + 1;
-  L.raw_stage_samples = c.decim * kTT + 2;
+  L.raw_stage_samples = raw_stage_samples(c, raw_bytes);
+  L.dstage_samples = chunk_stage_samples(c);   // one per decoder warp
   int o = 0;
-  L.o_raw = o; o = align_up(o + 2 * L.raw_stage_samples * 8, 16);
+  // the two raw stages; warp A1 later uses the region as its decoder stage
+  L.o_raw = o; o = align_up(o + std::max(2 * L.raw_stage_samples * raw_bytes, L.dstage_samples * 8), 16);
   L.o_tail_y = o; o = align_up(o + 2 * c.dc_length * 8, 16);
   L.o_ring_a = o; o += L.pas * kT2 * 4;
   L.seg_bytes = align_up(o, 16);
-  L.dstage_samples = chunk_stage_samples(c);   // one per decoder warp
   int off = 0;
   L.off_dA = off; off += L.pas * G * kPChainBuf * 4;
   L.off_dD = off; off += L.pds * 2 * G * kPChainBuf * 4;
@@ -282,14 +288,26 @@ void make_layout_pack(const RxConfig& c, int G, PackArgs& L)
 int pack_segments_per_cta(const rfid_b200_ctx* ctx, int nseg);
 
 typedef void (*fused_fn)(const FusedArgs);
-fused_fn pick_kernel(const RxConfig& c)
+template <class RAW>
+fused_fn pick_kernel_fmt(const RxConfig& c)
 {
   if (c.decim != 5) return nullptr;
   if (fast_path_ok(c)) {
-    if (c.mf_rem == 0 && c.mf_q == 5) return rx_fused_split_kernel<5, 5>;  // the reference configuration: 25 taps
-    return rx_fused_split_kernel<5, 0>;
+    if (c.mf_rem == 0 && c.mf_q == 5) return rx_fused_split_kernel<5, 5, RAW>;  // the reference configuration: 25 taps
+    return rx_fused_split_kernel<5, 0, RAW>;
   }
-  return rx_fused_kernel<5, 0>;  // long rings (raw rates above 5 MS/s) and any tap count
+  return rx_fused_kernel<5, 0, RAW>;  // long rings (raw rates above 5 MS/s) and any tap count
+}
+// the same choice for both capture formats
+fused_fn pick_kernel(const RxConfig& c, bool sc16 = false)
+{
+  return sc16 ? pick_kernel_fmt<RawSc16>(c) : pick_kernel_fmt<RawFc32>(c);
+}
+typedef void (*pack_fn)(const PackArgs);
+pack_fn pack_kernel(int pas, bool sc16)
+{
+  if (sc16) return pas == kPASMax ? rx_pack_kernel<5, 5, kPASMax, RawSc16> : rx_pack_kernel<5, 5, kPASMax - 1, RawSc16>;
+  return pas == kPASMax ? rx_pack_kernel<5, 5, kPASMax, RawFc32> : rx_pack_kernel<5, 5, kPASMax - 1, RawFc32>;
 }
 
 int grow(rfid_b200_ctx* ctx, void** p, size_t* have, size_t need)
@@ -390,7 +408,9 @@ int rfid_b200_create(const rfid_b200_params* p, rfid_b200_ctx** out)
   ctx->d_script_bytes = ctx->d_sim_res_bytes = ctx->d_sim_cnt_bytes = 0;
   ctx->h_stage[0] = ctx->h_stage[1] = nullptr; ctx->ev_stage[0] = ctx->ev_stage[1] = nullptr;
   memset(&ctx->layout, 0, sizeof(ctx->layout));
-  make_layout(cfg, ctx->layout);
+  memset(&ctx->layout_sc16, 0, sizeof(ctx->layout_sc16));
+  make_layout(cfg, (int)sizeof(RawFc32::T), ctx->layout);
+  make_layout(cfg, (int)sizeof(RawSc16::T), ctx->layout_sc16);
   cudaError_t e = cudaSetDevice(p->device);
   if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking);
   ctx->copy_stream = nullptr;
@@ -435,20 +455,23 @@ int rfid_b200_create(const rfid_b200_params* p, rfid_b200_ctx** out)
     int smem_max = 0;
     for (int G = 1; G <= kPMaxSeg; G++) {
       PackArgs pl;
-      make_layout_pack(cfg, G, pl);
+      make_layout_pack(cfg, G, (int)sizeof(RawFc32::T), pl);   // (sc16 stages are smaller)
       if (pl.smem_bytes > smem_max) smem_max = pl.smem_bytes;
     }
-    for (const void* fk : {(const void*)rx_pack_kernel<5, 5, kPASMax>, (const void*)rx_pack_kernel<5, 5, kPASMax - 1>}) {
+    for (const void* fk : {(const void*)pack_kernel(kPASMax, false), (const void*)pack_kernel(kPASMax - 1, false),
+                           (const void*)pack_kernel(kPASMax, true), (const void*)pack_kernel(kPASMax - 1, true)}) {
       if (e == cudaSuccess) e = cudaFuncSetAttribute(fk, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max);
       if (e == cudaSuccess)
         e = cudaFuncSetAttribute(fk, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
     }
   }
-  fused_fn fn = pick_kernel(cfg);
-  if (e == cudaSuccess && fn)
-    e = cudaFuncSetAttribute((const void*)fn, cudaFuncAttributeMaxDynamicSharedMemorySize, ctx->layout.smem_bytes);
-  if (e == cudaSuccess && fn)
-    e = cudaFuncSetAttribute((const void*)fn, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  for (int f = 0; f < 2; f++) {
+    fused_fn fn = pick_kernel(cfg, f == 1);
+    const int smem = (f == 1 ? ctx->layout_sc16 : ctx->layout).smem_bytes;
+    if (e == cudaSuccess && fn) e = cudaFuncSetAttribute((const void*)fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e == cudaSuccess && fn)
+      e = cudaFuncSetAttribute((const void*)fn, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  }
   if (e == cudaSuccess)
     e = cudaFuncSetAttribute((const void*)decode_block_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                              chunk_stage_samples(cfg) * 8);
@@ -528,30 +551,42 @@ int rfid_b200_kernel_time(rfid_b200_ctx* ctx, int reset, float* ms_total, int* l
 
 int rfid_b200_last_launch_count(const rfid_b200_ctx* ctx) { return ctx ? ctx->last_launches : RFID_B200_EINVAL; }
 
-static int decode_capture_impl(rfid_b200_ctx* ctx, const float* d_iq, size_t n_raw, const rfid_b200_segment* d_segs, int nseg,
-                               int max_windows_per_segment, rfid_b200_window_result* d_results, int32_t* d_counts,
-                               void* stream, int seg_base);
+// sc16 = false: d_iq holds fc32 samples (scale unused); true: sc16 samples, each converted with `scale`
+static int decode_capture_impl(rfid_b200_ctx* ctx, const void* d_iq, bool sc16, float scale, size_t n_raw,
+                               const rfid_b200_segment* d_segs, int nseg, int max_windows_per_segment,
+                               rfid_b200_window_result* d_results, int32_t* d_counts, void* stream, int seg_base);
+
+// an sc16 scale is a finite positive float
+static bool scale_ok(float scale) { return std::isfinite(scale) && scale > 0.f; }
 
 int rfid_b200_decode_capture(rfid_b200_ctx* ctx, const float* d_iq, size_t n_raw, const rfid_b200_segment* d_segs, int nseg,
                              int max_windows_per_segment, rfid_b200_window_result* d_results, int32_t* d_counts,
                              void* stream)
 {
-  return decode_capture_impl(ctx, d_iq, n_raw, d_segs, nseg, max_windows_per_segment, d_results, d_counts, stream, 0);
+  return decode_capture_impl(ctx, d_iq, false, 1.f, n_raw, d_segs, nseg, max_windows_per_segment, d_results, d_counts, stream, 0);
 }
 
-static int decode_capture_impl(rfid_b200_ctx* ctx, const float* d_iq, size_t n_raw, const rfid_b200_segment* d_segs, int nseg,
-                               int max_windows_per_segment, rfid_b200_window_result* d_results, int32_t* d_counts,
-                               void* stream, int seg_base)
+int rfid_b200_decode_capture_sc16(rfid_b200_ctx* ctx, const int16_t* d_iq, size_t n_raw, float scale,
+                                  const rfid_b200_segment* d_segs, int nseg, int max_windows_per_segment,
+                                  rfid_b200_window_result* d_results, int32_t* d_counts, void* stream)
+{
+  if (!scale_ok(scale)) return RFID_B200_EINVAL;
+  return decode_capture_impl(ctx, d_iq, true, scale, n_raw, d_segs, nseg, max_windows_per_segment, d_results, d_counts, stream, 0);
+}
+
+static int decode_capture_impl(rfid_b200_ctx* ctx, const void* d_iq, bool sc16, float scale, size_t n_raw,
+                               const rfid_b200_segment* d_segs, int nseg, int max_windows_per_segment,
+                               rfid_b200_window_result* d_results, int32_t* d_counts, void* stream, int seg_base)
 {
   if (!ctx || !d_iq || !d_segs || !d_results || !d_counts || nseg < 0 || max_windows_per_segment < 1) return RFID_B200_EINVAL;
   if ((reinterpret_cast<uintptr_t>(d_iq) & 15u) != 0) return RFID_B200_EINVAL;  // TMA bulk source alignment
   ctx->last_launches = 0;
   if (nseg == 0) return RFID_B200_OK;
-  fused_fn fn = pick_kernel(ctx->cfg);
+  fused_fn fn = pick_kernel(ctx->cfg, sc16);
   if (!fn) { ctx->last_error = "capture mode supports decim = 5 only in this build"; return RFID_B200_EINVAL; }
   CK(cudaSetDevice(ctx->device));
   cudaStream_t s = (cudaStream_t)stream;  // NULL = the (legacy) default stream, as documented
-  FusedArgs A = ctx->layout;
+  FusedArgs A = sc16 ? ctx->layout_sc16 : ctx->layout;
   const bool use_pack = pack_ok(ctx->cfg) && !ctx->pack_disabled;
   if (!use_pack) {
     // window scratch: one RN16 + one EPC window per segment (grown on demand; cudaMalloc synchronises, so a
@@ -560,7 +595,8 @@ static int decode_capture_impl(rfid_b200_ctx* ctx, const float* d_iq, size_t n_r
     if (rc) return rc;
   }
   A.win_scratch = reinterpret_cast<float2*>(ctx->d_win);
-  A.iq = reinterpret_cast<const float2*>(d_iq);
+  A.iq = d_iq;
+  A.scale = scale;
   A.n_raw = n_raw;
   A.segs = d_segs;
   A.nseg = nseg;
@@ -581,13 +617,13 @@ static int decode_capture_impl(rfid_b200_ctx* ctx, const float* d_iq, size_t n_r
   if (use_pack) {
     PackArgs P;
     memset(&P, 0, sizeof(P));
-    make_layout_pack(ctx->cfg, pack_segments_per_cta(ctx, nseg), P);
-    P.iq = A.iq; P.n_raw = A.n_raw; P.segs = A.segs; P.nseg = nseg; P.seg_base = seg_base; P.max_windows = A.max_windows;
+    make_layout_pack(ctx->cfg, pack_segments_per_cta(ctx, nseg), sc16 ? (int)sizeof(RawSc16::T) : (int)sizeof(RawFc32::T), P);
+    P.iq = A.iq; P.scale = scale; P.n_raw = A.n_raw; P.segs = A.segs; P.nseg = nseg; P.seg_base = seg_base; P.max_windows = A.max_windows;
     P.results = A.results; P.counts = A.counts; P.window_tap = A.window_tap; P.y_hist = reinterpret_cast<float2*>(ctx->d_yhist);
     P.cfg = ctx->cfg;
     // the y history belongs to one launch at a time: a launch on another stream than the previous one waits for it
     if (ctx->hist_used && ctx->hist_stream != s) CK(cudaStreamWaitEvent(s, ctx->ev_hist, 0));
-    auto kern = P.pas == kPASMax ? rx_pack_kernel<5, 5, kPASMax> : rx_pack_kernel<5, 5, kPASMax - 1>;
+    pack_fn kern = pack_kernel(P.pas, sc16);
     kern<<<(nseg + P.G - 1) / P.G, pack_threads(P.G), P.smem_bytes, s>>>(P);
     CK(cudaEventRecord(ctx->ev_hist, s));
     ctx->hist_stream = s; ctx->hist_used = true;
@@ -646,7 +682,7 @@ int rfid_b200_decode_capture_host(rfid_b200_ctx* ctx, const float* h_iq, size_t 
       CK(cudaEventRecord(ctx->ev_slice[k], ctx->copy_stream));
       CK(cudaStreamWaitEvent(s, ctx->ev_slice[k], 0));
     }
-    rc = decode_capture_impl(ctx, (const float*)ctx->d_iq, n_raw, (const rfid_b200_segment*)ctx->d_segs + b, e - b,
+    rc = decode_capture_impl(ctx, ctx->d_iq, false, 1.f, n_raw, (const rfid_b200_segment*)ctx->d_segs + b, e - b,
                              max_windows_per_segment, (rfid_b200_window_result*)ctx->d_res + (size_t)b * max_windows_per_segment,
                              (int32_t*)ctx->d_cnt + b, s, b);
     if (rc) return rc;
@@ -728,7 +764,7 @@ int rfid_b200_reduce_stats(const rfid_b200_ctx* ctx, const rfid_b200_window_resu
 
 namespace {
 
-constexpr size_t kUploadSamples = (size_t)1 << 21;  // 16 MiB per upload slice; multiple of kIngestChunk
+constexpr size_t kUploadBytes = (size_t)1 << 24;    // 16 MiB per upload slice: 2^21 fc32 or 2^22 sc16 samples, multiples of kIngestChunk
 constexpr size_t kLevelHead = (size_t)1 << 21;      // CW level is estimated on the head of the capture
 
 struct SegmenterCfg {
@@ -790,23 +826,38 @@ IngestPtrs ingest_ptrs(rfid_b200_ctx* ctx, long long n_chunks)
   return P;
 }
 
-int launch_level(rfid_b200_ctx* ctx, const float2* d_iq, size_t n_raw, const SegmenterCfg& sc, const IngestPtrs& P, cudaStream_t s)
+// the capture in device memory: its samples and their format (RAW of rx_common.cuh)
+struct DevCapture {
+  const void* iq;
+  bool sc16;
+  float scale;   // sc16 only
+};
+
+int launch_level(rfid_b200_ctx* ctx, const DevCapture& X, size_t n_raw, const SegmenterCfg& sc, const IngestPtrs& P, cudaStream_t s)
 {
   const unsigned long long n0 = n_raw < kLevelHead ? n_raw : kLevelHead;
-  ingest_level_partial<<<kLevelBlocks, kLevelThreads, 0, s>>>(d_iq, n0, P.partial);
+  if (X.sc16)
+    ingest_level_partial<RawSc16><<<kLevelBlocks, kLevelThreads, 0, s>>>(static_cast<const uint32_t*>(X.iq), X.scale, n0, P.partial);
+  else
+    ingest_level_partial<RawFc32><<<kLevelBlocks, kLevelThreads, 0, s>>>(static_cast<const float2*>(X.iq), 1.f, n0, P.partial);
   ingest_level_final<<<1, 32, 0, s>>>(P.partial, n0, sc.level_frac, P.tot);
   CK(cudaGetLastError());
   ctx->last_launches += 2;
   return RFID_B200_OK;
 }
 
-int launch_mask(rfid_b200_ctx* ctx, const float2* d_iq, size_t n_raw, long long first_chunk, long long n, const IngestPtrs& P,
+int launch_mask(rfid_b200_ctx* ctx, const DevCapture& X, size_t n_raw, long long first_chunk, long long n, const IngestPtrs& P,
                 cudaStream_t s)
 {
   if (n <= 0) return RFID_B200_OK;
   long long blocks = (n + 7) / 8;
   if (blocks > ctx->sm_count * 8) blocks = ctx->sm_count * 8;
-  ingest_mask<<<(unsigned)blocks, 256, 0, s>>>(d_iq, n_raw, first_chunk, n, P.tot, P.mask, P.chunk_last, P.chunk_falls);
+  if (X.sc16)
+    ingest_mask<RawSc16><<<(unsigned)blocks, 256, 0, s>>>(static_cast<const uint32_t*>(X.iq), X.scale, n_raw, first_chunk, n,
+                                                          P.tot, P.mask, P.chunk_last, P.chunk_falls);
+  else
+    ingest_mask<RawFc32><<<(unsigned)blocks, 256, 0, s>>>(static_cast<const float2*>(X.iq), 1.f, n_raw, first_chunk, n, P.tot,
+                                                          P.mask, P.chunk_last, P.chunk_falls);
   CK(cudaGetLastError());
   ctx->last_launches += 1;
   return RFID_B200_OK;
@@ -883,10 +934,12 @@ void rfid_b200_default_segmenter(rfid_b200_segmenter* sp)
   sp->commands_per_segment = 2;            // RN16 window + EPC window
 }
 
-int rfid_b200_segment_capture(rfid_b200_ctx* ctx, const float* d_iq, size_t n_raw, const rfid_b200_segmenter* sp,
-                              rfid_b200_segment* h_segs, int capacity, int* nseg, void* stream)
+}  // extern "C"
+
+static int segment_capture_impl(rfid_b200_ctx* ctx, const DevCapture& X, size_t n_raw, const rfid_b200_segmenter* sp,
+                                rfid_b200_segment* h_segs, int capacity, int* nseg, void* stream)
 {
-  if (!ctx || !d_iq || !h_segs || !nseg || capacity < 0) return RFID_B200_EINVAL;
+  if (!ctx || !X.iq || !h_segs || !nseg || capacity < 0) return RFID_B200_EINVAL;
   *nseg = 0;
   SegmenterCfg sc;
   int rc = resolve_segmenter(ctx, sp, sc);
@@ -898,35 +951,37 @@ int rfid_b200_segment_capture(rfid_b200_ctx* ctx, const float* d_iq, size_t n_ra
   if ((rc = ingest_alloc(ctx, n_raw, sc, n_chunks, burst_cap))) return rc;
   const IngestPtrs P = ingest_ptrs(ctx, n_chunks);
   cudaStream_t s = (cudaStream_t)stream;
-  const float2* iq = reinterpret_cast<const float2*>(d_iq);
   ctx->last_launches = 0;
-  if ((rc = launch_level(ctx, iq, n_raw, sc, P, s))) return rc;
-  if ((rc = launch_mask(ctx, iq, n_raw, 0, n_chunks, P, s))) return rc;
+  if ((rc = launch_level(ctx, X, n_raw, sc, P, s))) return rc;
+  if ((rc = launch_mask(ctx, X, n_raw, 0, n_chunks, P, s))) return rc;
   IngestTotals tot;
   if ((rc = finish_bursts(ctx, n_chunks, burst_cap, sc, P, s, tot))) return rc;
   return build_segments(ctx, ctx->h_bursts, tot.n_falls, n_raw, sc, h_segs, capacity, nseg);
 }
 
-int rfid_b200_ingest_capture_host(rfid_b200_ctx* ctx, const float* h_iq, size_t n_raw, const rfid_b200_segmenter* sp,
-                                  int max_windows_per_segment, rfid_b200_segment* h_segs, int seg_capacity, int* nseg,
-                                  rfid_b200_window_result* h_results, int32_t* h_counts)
+// h_iq: n_raw samples of sample_bytes each (8 fc32, 4 sc16)
+static int ingest_capture_host_impl(rfid_b200_ctx* ctx, const void* h_iq, bool sc16, float scale, size_t n_raw,
+                                    const rfid_b200_segmenter* sp, int max_windows_per_segment, rfid_b200_segment* h_segs,
+                                    int seg_capacity, int* nseg, rfid_b200_window_result* h_results, int32_t* h_counts)
 {
   if (!ctx || !h_iq || !h_segs || !nseg || !h_results || !h_counts || seg_capacity < 0 || max_windows_per_segment < 1)
     return RFID_B200_EINVAL;
+  const size_t sb = sc16 ? sizeof(RawSc16::T) : sizeof(RawFc32::T);   // bytes per sample
+  const size_t slice_samples = kUploadBytes / sb;
   *nseg = 0;
   SegmenterCfg sc;
   int rc = resolve_segmenter(ctx, sp, sc);
   if (rc) return rc;
   if (n_raw == 0) return RFID_B200_OK;
-  if (!pick_kernel(ctx->cfg)) { ctx->last_error = "capture mode supports decim = 5 only in this build"; return RFID_B200_EINVAL; }
+  if (!pick_kernel(ctx->cfg, sc16)) { ctx->last_error = "capture mode supports decim = 5 only in this build"; return RFID_B200_EINVAL; }
   CK(cudaSetDevice(ctx->device));
   long long n_chunks;
   unsigned int burst_cap;
   if ((rc = ingest_alloc(ctx, n_raw, sc, n_chunks, burst_cap))) return rc;
-  if ((rc = grow(ctx, &ctx->d_iq, &ctx->d_iq_bytes, n_raw * 8 + 16))) return rc;
+  if ((rc = grow(ctx, &ctx->d_iq, &ctx->d_iq_bytes, n_raw * sb + 16))) return rc;
   const IngestPtrs P = ingest_ptrs(ctx, n_chunks);
   cudaStream_t s = ctx->stream;
-  const float2* d_iq = reinterpret_cast<const float2*>(ctx->d_iq);
+  const DevCapture X{ctx->d_iq, sc16, scale};
 
   // pageable sources go through two pinned staging slices so the host memcpy of slice k+1 overlaps the DMA of
   // slice k; pinned (registered) sources are DMA'd directly.  The threshold pass runs behind each slice.
@@ -936,7 +991,7 @@ int rfid_b200_ingest_capture_host(rfid_b200_ctx* ctx, const float* h_iq, size_t 
   if (!pinned) {
     for (int b = 0; b < 2; b++) {
       if (!ctx->h_stage[b]) {
-        if (cudaHostAlloc(&ctx->h_stage[b], kUploadSamples * 8, cudaHostAllocDefault) != cudaSuccess) {
+        if (cudaHostAlloc(&ctx->h_stage[b], kUploadBytes, cudaHostAllocDefault) != cudaSuccess) {
           cudaGetLastError();
           return RFID_B200_ENOMEM;
         }
@@ -947,23 +1002,24 @@ int rfid_b200_ingest_capture_host(rfid_b200_ctx* ctx, const float* h_iq, size_t 
   ctx->last_launches = 0;
   int launches = 0;
   size_t slice = 0;
-  for (size_t off = 0; off < n_raw; off += kUploadSamples, slice++) {
-    const size_t n = n_raw - off < kUploadSamples ? n_raw - off : kUploadSamples;
-    const float* src = h_iq + 2 * off;
+  for (size_t off = 0; off < n_raw; off += slice_samples, slice++) {
+    const size_t n = n_raw - off < slice_samples ? n_raw - off : slice_samples;
+    const char* src = static_cast<const char*>(h_iq) + off * sb;
     if (!pinned) {
       const int b = (int)(slice & 1);
       if (slice >= 2) CK(cudaEventSynchronize(ctx->ev_stage[b]));
-      memcpy(ctx->h_stage[b], src, n * 8);
-      CK(cudaMemcpyAsync((char*)ctx->d_iq + off * 8, ctx->h_stage[b], n * 8, cudaMemcpyHostToDevice, s));
+      memcpy(ctx->h_stage[b], src, n * sb);
+      CK(cudaMemcpyAsync((char*)ctx->d_iq + off * sb, ctx->h_stage[b], n * sb, cudaMemcpyHostToDevice, s));
       CK(cudaEventRecord(ctx->ev_stage[b], s));
     } else {
-      CK(cudaMemcpyAsync((char*)ctx->d_iq + off * 8, src, n * 8, cudaMemcpyHostToDevice, s));
+      CK(cudaMemcpyAsync((char*)ctx->d_iq + off * sb, src, n * sb, cudaMemcpyHostToDevice, s));
     }
-    if (off == 0 && (rc = launch_level(ctx, d_iq, n_raw, sc, P, s))) return rc;
+    // (the first slice holds the level's head: kLevelHead <= 2^21 samples)
+    if (off == 0 && (rc = launch_level(ctx, X, n_raw, sc, P, s))) return rc;
     const long long first = (long long)(off / kIngestChunk);
     const long long cnt = (long long)((n + kIngestChunk - 1) / kIngestChunk);
-    // the mask kernel treats samples beyond `off + n` as not yet present: pass the uploaded extent as n_raw
-    if ((rc = launch_mask(ctx, d_iq, off + n, first, cnt, P, s))) return rc;
+    // the mask kernel treats samples beyond `off + n` as not yet present: pass the uploaded extent (samples) as n_raw
+    if ((rc = launch_mask(ctx, X, off + n, first, cnt, P, s))) return rc;
   }
   IngestTotals tot;
   if ((rc = finish_bursts(ctx, n_chunks, burst_cap, sc, P, s, tot))) return rc;
@@ -977,14 +1033,49 @@ int rfid_b200_ingest_capture_host(rfid_b200_ctx* ctx, const float* h_iq, size_t 
   if ((rc = grow(ctx, &ctx->d_cnt, &ctx->d_cnt_bytes, (size_t)ns * 4))) return rc;
   CK(cudaMemcpyAsync(ctx->d_segs, h_segs, (size_t)ns * sizeof(rfid_b200_segment), cudaMemcpyHostToDevice, s));
   CK(cudaMemsetAsync(ctx->d_res, 0, res_bytes, s));
-  rc = rfid_b200_decode_capture(ctx, (const float*)ctx->d_iq, n_raw, (const rfid_b200_segment*)ctx->d_segs, ns,
-                                max_windows_per_segment, (rfid_b200_window_result*)ctx->d_res, (int32_t*)ctx->d_cnt, s);
+  rc = decode_capture_impl(ctx, ctx->d_iq, sc16, scale, n_raw, (const rfid_b200_segment*)ctx->d_segs, ns,
+                           max_windows_per_segment, (rfid_b200_window_result*)ctx->d_res, (int32_t*)ctx->d_cnt, s, 0);
   if (rc) return rc;
   ctx->last_launches += launches;
   CK(cudaMemcpyAsync(h_results, ctx->d_res, res_bytes, cudaMemcpyDeviceToHost, s));
   CK(cudaMemcpyAsync(h_counts, ctx->d_cnt, (size_t)ns * 4, cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
   return RFID_B200_OK;
+}
+
+extern "C" {
+
+int rfid_b200_segment_capture(rfid_b200_ctx* ctx, const float* d_iq, size_t n_raw, const rfid_b200_segmenter* sp,
+                              rfid_b200_segment* h_segs, int capacity, int* nseg, void* stream)
+{
+  return segment_capture_impl(ctx, DevCapture{d_iq, false, 1.f}, n_raw, sp, h_segs, capacity, nseg, stream);
+}
+
+int rfid_b200_segment_capture_sc16(rfid_b200_ctx* ctx, const int16_t* d_iq, size_t n_raw, float scale,
+                                   const rfid_b200_segmenter* sp, rfid_b200_segment* h_segs, int capacity, int* nseg,
+                                   void* stream)
+{
+  if (nseg) *nseg = 0;
+  if (!scale_ok(scale) || (reinterpret_cast<uintptr_t>(d_iq) & 15u) != 0) return RFID_B200_EINVAL;
+  return segment_capture_impl(ctx, DevCapture{d_iq, true, scale}, n_raw, sp, h_segs, capacity, nseg, stream);
+}
+
+int rfid_b200_ingest_capture_host(rfid_b200_ctx* ctx, const float* h_iq, size_t n_raw, const rfid_b200_segmenter* sp,
+                                  int max_windows_per_segment, rfid_b200_segment* h_segs, int seg_capacity, int* nseg,
+                                  rfid_b200_window_result* h_results, int32_t* h_counts)
+{
+  return ingest_capture_host_impl(ctx, h_iq, false, 1.f, n_raw, sp, max_windows_per_segment, h_segs, seg_capacity, nseg,
+                                  h_results, h_counts);
+}
+
+int rfid_b200_ingest_capture_host_sc16(rfid_b200_ctx* ctx, const int16_t* h_iq, size_t n_raw, float scale,
+                                       const rfid_b200_segmenter* sp, int max_windows_per_segment, rfid_b200_segment* h_segs,
+                                       int seg_capacity, int* nseg, rfid_b200_window_result* h_results, int32_t* h_counts)
+{
+  if (nseg) *nseg = 0;
+  if (!scale_ok(scale)) return RFID_B200_EINVAL;
+  return ingest_capture_host_impl(ctx, h_iq, true, scale, n_raw, sp, max_windows_per_segment, h_segs, seg_capacity, nseg,
+                                  h_results, h_counts);
 }
 
 // ------------------------------------------------------------------ TX synthesiser + slot simulator (SURVEY 8f-1)

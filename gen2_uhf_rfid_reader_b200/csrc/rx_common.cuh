@@ -292,62 +292,113 @@ __device__ __forceinline__ void chain_inplace(float* buf, int n, float& acc)
   }
 }
 
-// raw tile geometry: segment-relative index of the first sample held in the stage buffer
-template <int DECIM>
+// ---- raw sample formats.  Every capture kernel is instantiated for each: its raw stages hold the capture's own elements,
+// and every sample is converted to float2 as P1 reads it, so the stages move the capture's bytes and no more.
+struct RawFc32 {               // interleaved float32 I, Q (8 B per sample)
+  typedef float2 T;
+  static constexpr int kBytes = 8;
+  static __device__ __forceinline__ float2 cvt(float2 v, float) { return v; }
+  static __device__ __forceinline__ float2 ldcs(const float2* p) { return __ldcs(p); }
+};
+struct RawSc16 {               // interleaved int16 I, Q (UHD "sc16", 4 B per sample): I in the low half-word
+  typedef uint32_t T;
+  static constexpr int kBytes = 4;
+  // ((float)I * scale, (float)Q * scale): one round-to-nearest multiply per component, as np.float32(i) * np.float32(scale)
+  // (int16 -> float is exact; I2F measured faster than the exact IADD + FADD form, tests/cuda/sc16_harness.cu)
+  static __device__ __forceinline__ float2 cvt(uint32_t v, float scale)
+  {
+    const int i = (short)(v & 0xFFFFu), q = (int)v >> 16;
+    return make_float2(f_mul((float)i, scale), f_mul((float)q, scale));
+  }
+  static __device__ __forceinline__ uint32_t ldcs(const uint32_t* p) { return __ldcs(p); }
+};
+// samples per 16-byte TMA granule: a stage starts at a multiple of this absolute sample index
+template <class RAW>
+__host__ __device__ constexpr int raw_granule() { return 16 / RAW::kBytes; }
+
+// N consecutive sc16 samples stage[st .. st + N) of one lane (st mod 4 the same for the whole warp): the aligned 16-byte
+// loads of the words around them, then a shift by st mod 4 words in two select steps (by 2, by 1), so that every stage
+// residue takes the vector path.  Reads up to 6 words past the run (the stages have that room: kSc16StagePad).
+template <int N>
+__device__ __forceinline__ void sc16_run(const uint32_t* stage, int st, uint32_t (&x)[N])
+{
+  constexpr int NQ = (N + 6) / 4;   // granules covering words st & ~3 .. (st & ~3) + 3 + N
+  const int r = st & 3;
+  uint32_t w[4 * NQ];
+  const uint4* p = reinterpret_cast<const uint4*>(stage + (st & ~3));
+#pragma unroll
+  for (int j = 0; j < NQ; j++) {
+    const uint4 v = p[j];
+    w[4 * j] = v.x; w[4 * j + 1] = v.y; w[4 * j + 2] = v.z; w[4 * j + 3] = v.w;
+  }
+  uint32_t s[N + 1];
+#pragma unroll
+  for (int j = 0; j < N + 1; j++) s[j] = (r & 2) ? w[j + 2] : w[j];
+#pragma unroll
+  for (int j = 0; j < N; j++) x[j] = (r & 1) ? s[j + 1] : s[j];
+}
+constexpr int kSc16StagePad = 8;    // samples of an sc16 raw stage beyond a tile's D*kTT: granule alignment + read-ahead
+
+// raw tile geometry: segment-relative index of the first sample held in the stage buffer (moved down to a 16-byte
+// aligned absolute index)
+template <int DECIM, class RAW>
 __device__ __forceinline__ long long tile_load_start(unsigned long long seg_off, int k)
 {
   long long lo = (long long)DECIM * k * kTT - (DECIM - 1);
   if (lo < 0) lo = 0;
   long long abs_lo = (long long)seg_off + lo;
-  abs_lo &= ~1ll;  // 16-byte aligned source
+  abs_lo &= ~(long long)(raw_granule<RAW>() - 1);  // 16-byte aligned source
   return abs_lo - (long long)seg_off;
 }
 
 // the copy of raw tile k of segment sg (any tile; iq holds n_raw samples)
-template <int DECIM>
-__device__ __forceinline__ void issue_tile_load(const float2* iq, unsigned long long n_raw, const rfid_b200_segment& sg,
-                                                int k, float2* stage, uint64_t* bar)
+template <int DECIM, class RAW>
+__device__ __forceinline__ void issue_tile_load(const typename RAW::T* iq, unsigned long long n_raw, const rfid_b200_segment& sg,
+                                                int k, typename RAW::T* stage, uint64_t* bar)
 {
-  const long long start = tile_load_start<DECIM>(sg.offset, k);  // may be -1
+  constexpr int E = raw_granule<RAW>();
+  const long long start = tile_load_start<DECIM, RAW>(sg.offset, k);  // may be up to E-1 below the segment
   long long hi = (long long)DECIM * ((long long)k * kTT + kTT - 1);
   if (hi > (long long)sg.length - 1) hi = (long long)sg.length - 1;
   long long count = hi - start + 1;  // samples start..hi
-  long long count_al = (count + 1) & ~1ll;
+  long long count_al = (count + E - 1) & ~(long long)(E - 1);
   const long long abs_start = (long long)sg.offset + start;
-  float2 tail = make_float2(0.f, 0.f);
-  bool patch = false;
   if ((unsigned long long)(abs_start + count_al) > n_raw) {
-    // the rounded-up copy would run one sample past the capture buffer: copy an even count and
-    // fetch the last sample with a plain load
-    count_al -= 2;
-    tail = iq[abs_start + count - 1];
-    patch = true;
+    // the rounded-up copy would run past the capture buffer: copy whole granules and fetch the last (at most E-1)
+    // samples with plain loads
+    count_al = count & ~(long long)(E - 1);
+#pragma unroll
+    for (int j = 0; j < E - 1; j++)
+      if (count_al + j < count) stage[count_al + j] = iq[abs_start + count_al + j];
   }
-  const uint32_t bytes = (uint32_t)(count_al * 8);
-  if (patch) stage[count - 1] = tail;
+  const uint32_t bytes = (uint32_t)(count_al * RAW::kBytes);
   mbar_arrive_expect_tx(bar, bytes);
   if (bytes) tma_load_1d(stage, iq + abs_start, bytes, bar);
 }
 
-// Tile k >= 1 starts at raw sample D*kTT*k - (D-1) of the segment, moved down to an even absolute index (16-byte TMA
-// source); tile 0 starts at the segment's first (even-aligned) sample.  Tiles 1 .. n-1 are interior: their last sample
-// D*(k*kTT + kTT-1) exists and the rounded-up copy stays inside the capture, so each is `bytes` bytes from
-// src + D*kTT*k.  The other tiles go through issue_tile_load.
+// Tile k >= 1 starts at raw sample D*kTT*k - (D-1) of the segment, moved down to a 16-byte aligned absolute index (by
+// r = offset mod E samples, E = raw_granule); tile 0 starts at the segment's first (aligned) sample.  Tiles 1 .. n-1 are
+// interior: their last sample D*(k*kTT + kTT-1) exists and the rounded-up copy stays inside the capture, so each is
+// `bytes` bytes from src + D*kTT*k.  The other tiles go through issue_tile_load.
+template <class T>
 struct InteriorTiles {
-  const float2* src;
+  const T* src;
   uint32_t bytes;
   int n;
 };
-template <int DECIM>
-__device__ __forceinline__ InteriorTiles interior_tiles(const float2* iq, unsigned long long n_raw,
-                                                        const rfid_b200_segment& sg, int ntiles)
+template <int DECIM, class RAW>
+__device__ __forceinline__ InteriorTiles<typename RAW::T> interior_tiles(const typename RAW::T* iq, unsigned long long n_raw,
+                                                                         const rfid_b200_segment& sg, int ntiles)
 {
-  const int odd = (int)(sg.offset & 1ull);
-  InteriorTiles t;
-  t.src = iq + sg.offset - (DECIM - 1) - odd;
-  t.bytes = (uint32_t)((DECIM * kTT + 2 * odd) * 8);
+  constexpr int E = raw_granule<RAW>();
+  static_assert((DECIM - 1) % E == 0, "interior tiles start on a granule");
+  const int r = (int)(sg.offset & (unsigned long long)(E - 1));
+  const int span = DECIM * kTT + ((r + E - 1) & ~(E - 1));   // samples copied per interior tile
+  InteriorTiles<typename RAW::T> t;
+  t.src = iq + sg.offset - (DECIM - 1) - r;
+  t.bytes = (uint32_t)(span * RAW::kBytes);
   const long long by_len = ((long long)sg.length - 1 - (long long)DECIM * (kTT - 1)) / ((long long)DECIM * kTT);
-  const long long room = (long long)n_raw - (long long)sg.offset + (DECIM - 1) + odd - (DECIM * kTT + 2 * odd);
+  const long long room = (long long)n_raw - (long long)sg.offset + (DECIM - 1) + r - span;
   const long long by_buf = room >= 0 ? room / ((long long)DECIM * kTT) : -1;
   long long f = (by_len < by_buf ? by_len : by_buf) + 1;
   if (sg.length < (unsigned)(DECIM * kTT)) f = 0;

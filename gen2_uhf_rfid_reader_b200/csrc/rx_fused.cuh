@@ -75,7 +75,7 @@ __device__ __forceinline__ void bar_sync_workers()
 }
 
 struct FusedArgs {
-  const float2* iq;              // raw capture (device), 16-byte aligned
+  const void* iq;                // raw capture (device, RAW::T[n_raw]), 16-byte aligned
   unsigned long long n_raw;      // total samples in the capture buffer
   const rfid_b200_segment* segs;
   int nseg;
@@ -98,6 +98,7 @@ struct FusedArgs {
   int off_etile;                 // float[kTileStages][2][kTT] (+pad)       (fast path: workers' DC-ring differences)
   int off_snap;                  // float2[dc_length]: dc ring snapshot taken when the gate opens (fast path)
   int smem_bytes;
+  float scale;                   // sc16 captures: the int16 -> float factor (RawSc16::cvt)
 };
 
 struct TileEvent {
@@ -118,7 +119,7 @@ struct FusedShared {
 // MFQ > 0: ntaps == MFQ * DECIM (compile-time unrolled block sums); MFQ == 0: generic ntaps.
 // This kernel keeps explicit amplitude / closed-sample rings of any length: it serves every rate whose 250 us window is
 // longer than a tile (raw rates of 2.6 MS/s and up); rx_fused_split_kernel is the fast path below that.
-template <int DECIM, int MFQ>
+template <int DECIM, int MFQ, class RAW>
 __global__ void __launch_bounds__(kFusedThreads, 8) rx_fused_kernel(const FusedArgs A)
 {
   extern __shared__ __align__(128) unsigned char smem[];
@@ -132,7 +133,9 @@ __global__ void __launch_bounds__(kFusedThreads, 8) rx_fused_kernel(const FusedA
   const int n_out = (int)(sg.length / DECIM);
   const int ntiles = (n_out + kTT - 1) / kTT;
 
-  float2* raw = reinterpret_cast<float2*>(smem + A.off_raw);
+  typedef typename RAW::T RawT;
+  const RawT* const iq = static_cast<const RawT*>(A.iq);
+  RawT* raw = reinterpret_cast<RawT*>(smem + A.off_raw);
   float2* bhist = reinterpret_cast<float2*>(smem + A.off_bhist);
   float2* phist = bhist + A.bhist_size;
   float* ahist = reinterpret_cast<float*>(smem + A.off_ahist);
@@ -165,16 +168,16 @@ __global__ void __launch_bounds__(kFusedThreads, 8) rx_fused_kernel(const FusedA
     const int wt = (warp - 1) * 32 + lane;
     if (wt == 0) {
       for (int k = 0; k < kRawStages && k < ntiles; k++)
-        issue_tile_load<DECIM>(A.iq, A.n_raw, sg, k, raw + (size_t)k * A.raw_stage_samples, &B.raw_full[k]);
+        issue_tile_load<DECIM, RAW>(iq, A.n_raw, sg, k, raw + (size_t)k * A.raw_stage_samples, &B.raw_full[k]);
     }
     const int bmask = A.bhist_size - 1, amask = A.ahist_size - 1;
     const float winlen_f = (float)C.win_length;
     PH_DECL
     for (int k = 0; k < ntiles; k++) {
       const int rs = k % kRawStages, ts = k % kTileStages;
-      const float2* stage = raw + (size_t)rs * A.raw_stage_samples;
+      const RawT* stage = raw + (size_t)rs * A.raw_stage_samples;
       // stage index of raw sample x[D*n - (D-1) + j] for tile-local output t:  D*t - (D-1) + j - delta
-      const int delta = (int)(tile_load_start<DECIM>(sg.offset, k) - (long long)DECIM * k * kTT);
+      const int delta = (int)(tile_load_start<DECIM, RAW>(sg.offset, k) - (long long)DECIM * k * kTT);
       const int nvalid = min(kTT, n_out - k * kTT);
       PH_MARK(0)
       mbar_wait(&B.raw_full[rs], (k / kRawStages) & 1);
@@ -191,7 +194,7 @@ __global__ void __launch_bounds__(kFusedThreads, 8) rx_fused_kernel(const FusedA
           for (int j = 0; j < DECIM; j++) {
             // only the very first block of a segment reaches before sample 0 (reads as +0)
             const bool before = (k == 0) && (DECIM * t - (DECIM - 1) + j < 0);
-            x[j] = before ? make_float2(0.f, 0.f) : stage[base + j];
+            x[j] = before ? make_float2(0.f, 0.f) : RAW::cvt(stage[base + j], A.scale);
           }
           float2 b = x[0];
 #pragma unroll
@@ -214,7 +217,7 @@ __global__ void __launch_bounds__(kFusedThreads, 8) rx_fused_kernel(const FusedA
       PH_MARK(2)
       bar_sync_workers();  // raw stage rs fully consumed, block sums visible
       if (wt == 0 && k + kRawStages < ntiles)
-        issue_tile_load<DECIM>(A.iq, A.n_raw, sg, k + kRawStages, raw + (size_t)rs * A.raw_stage_samples, &B.raw_full[rs]);
+        issue_tile_load<DECIM, RAW>(iq, A.n_raw, sg, k + kRawStages, raw + (size_t)rs * A.raw_stage_samples, &B.raw_full[rs]);
       PH_MARK(3)
       if (k >= kTileStages) bar_sync_stage<BAR_TILE_EMPTY>(ts, 96);  // the sequencer is done with tile k - 3
       PH_MARK(4)

@@ -84,7 +84,7 @@ __device__ __forceinline__ void mbar_wait_hot(uint64_t* bar, uint32_t parity)
   mbar_wait_relaxed(bar, parity, 2000);  // try_wait with a suspend hint: the hardware parks the warp until the phase flips
 }
 
-template <int DECIM, int MFQ>
+template <int DECIM, int MFQ, class RAW>
 __global__ void __launch_bounds__(kSplitThreads, 7) rx_fused_split_kernel(const FusedArgs A)
 {
   extern __shared__ __align__(128) unsigned char smem[];
@@ -125,7 +125,8 @@ __global__ void __launch_bounds__(kSplitThreads, 7) rx_fused_split_kernel(const 
   const int n_out = (int)(sg.length / DECIM);
   const int ntiles = (n_out + kTT - 1) / kTT;
 
-  float2* raw = reinterpret_cast<float2*>(smem + A.off_raw);
+  typedef typename RAW::T RawT;
+  RawT* raw = reinterpret_cast<RawT*>(smem + A.off_raw);
   float2* bhist = reinterpret_cast<float2*>(smem + A.off_bhist);
   float2* phist = bhist + A.bhist_size;
   float2* ring_y = reinterpret_cast<float2*>(smem + A.off_tile_y);   // [kRing]
@@ -157,16 +158,18 @@ __global__ void __launch_bounds__(kSplitThreads, 7) rx_fused_split_kernel(const 
   if (role >= 2 && role < 2 + kSWWarps) {
     // =========================================================== workers
     const int wt = (role - 2) * 32 + lane;
-    // raw tile geometry (interior_tiles): tile k >= 1 starts at raw sample D*kTT*k - (D-1) - odd of the segment
-    const int odd = (int)(sg.offset & 1ull);
-    const InteriorTiles fast = interior_tiles<DECIM>(A.iq, A.n_raw, sg, ntiles);
+    // raw tile geometry (interior_tiles): tile k >= 1 starts at raw sample D*kTT*k - (D-1) - odd of the segment, odd =
+    // the offset's residue modulo the 16-byte granule
+    const RawT* const iq = static_cast<const RawT*>(A.iq);
+    const int odd = (int)(sg.offset & (unsigned long long)(raw_granule<RAW>() - 1));
+    const InteriorTiles<RawT> fast = interior_tiles<DECIM, RAW>(iq, A.n_raw, sg, ntiles);
     auto load_tile = [&](int k, int rs_) {
-      float2* dst = raw + (size_t)rs_ * A.raw_stage_samples;
+      RawT* dst = raw + (size_t)rs_ * A.raw_stage_samples;
       if (k >= 1 && k < fast.n) {
         mbar_arrive_expect_tx(&B.raw_full[rs_], fast.bytes);
         tma_load_1d(dst, fast.src + (size_t)k * (DECIM * kTT), fast.bytes, &B.raw_full[rs_]);
       } else {
-        issue_tile_load<DECIM>(A.iq, A.n_raw, sg, k, dst, &B.raw_full[rs_]);
+        issue_tile_load<DECIM, RAW>(iq, A.n_raw, sg, k, dst, &B.raw_full[rs_]);
       }
     };
     if (wt == 0) {
@@ -181,7 +184,7 @@ __global__ void __launch_bounds__(kSplitThreads, 7) rx_fused_split_kernel(const 
     int rs = 0, ts = 0;                  // k % kRawStages, k % kS
     uint32_t raw_par = 0, free_par = 1;  // (k / kRawStages) & 1, ((k / kS) & 1) ^ 1
     for (int k = 0; k < ntiles; k++) {
-      const float2* stage = raw + (size_t)rs * A.raw_stage_samples;
+      const RawT* stage = raw + (size_t)rs * A.raw_stage_samples;
       const int delta = -odd - (k > 0 ? DECIM - 1 : 0);  // tile_load_start(k) - D*kTT*k
       const int nvalid = min(kTT, n_out - k * kTT);
       PH_MARK(0)
@@ -200,7 +203,16 @@ __global__ void __launch_bounds__(kSplitThreads, 7) rx_fused_split_kernel(const 
 #pragma unroll
         for (int h = 0; h < Q; h += 2) {
           float2 x[2 * DECIM];
-          if (odd == 0 && k > 0) {
+          if constexpr (RAW::kBytes == 4) {
+            uint32_t xs[2 * DECIM];   // interior half-tiles: two outputs' raw samples, one vector run
+            if (k > 0) sc16_run(stage, base + DECIM * h, xs);
+#pragma unroll
+            for (int j = 0; j < 2 * DECIM; j++) {
+              const bool before = (k == 0) && (DECIM * (t0 + h) - (DECIM - 1) + j < 0);  // before sample 0 of the segment: +0
+              x[j] = before ? make_float2(0.f, 0.f)
+                            : RAW::cvt(k > 0 ? xs[j] : stage[base + DECIM * h + j], A.scale);
+            }
+          } else if (odd == 0 && k > 0) {
             const float4* p4 = reinterpret_cast<const float4*>(stage + base + DECIM * h);
 #pragma unroll
             for (int j = 0; j < DECIM; j++) {
@@ -328,10 +340,10 @@ __global__ void __launch_bounds__(kSplitThreads, 7) rx_fused_split_kernel(const 
             float2 x[DECIM];
             if (k == 0 && t == 0) {  // the segment's very first block reaches before sample 0: those read as +0
   #pragma unroll
-              for (int j = 0; j < DECIM; j++) x[j] = j < DECIM - 1 ? make_float2(0.f, 0.f) : stage[base + j];
+              for (int j = 0; j < DECIM; j++) x[j] = j < DECIM - 1 ? make_float2(0.f, 0.f) : RAW::cvt(stage[base + j], A.scale);
             } else {
   #pragma unroll
-              for (int j = 0; j < DECIM; j++) x[j] = stage[base + j];
+              for (int j = 0; j < DECIM; j++) x[j] = RAW::cvt(stage[base + j], A.scale);
             }
             float2 b = x[0];
   #pragma unroll

@@ -41,14 +41,17 @@ struct IngestTotals {
   float level;                    // CW level estimate
 };
 
-__global__ void __launch_bounds__(kLevelThreads) ingest_level_partial(const float2* __restrict__ iq, unsigned long long n0,
-                                                                     double* __restrict__ partial)
+// RAW: the capture's sample format (rx_common.cuh); every sample is converted (RAW::cvt, `scale`) before it is used, so
+// an sc16 capture gives the level, masks and segment table of its fc32 conversion
+template <class RAW>
+__global__ void __launch_bounds__(kLevelThreads) ingest_level_partial(const typename RAW::T* __restrict__ iq, float scale,
+                                                                     unsigned long long n0, double* __restrict__ partial)
 {
   __shared__ double s_w[kLevelThreads / 32];
   double acc = 0.0;
   for (unsigned long long i = (unsigned long long)blockIdx.x * kLevelThreads + threadIdx.x; i < n0;
        i += (unsigned long long)kLevelBlocks * kLevelThreads) {
-    const float2 v = iq[i];
+    const float2 v = RAW::cvt(iq[i], scale);
     acc += (double)sqrtf(v.x * v.x + v.y * v.y);
   }
   for (int o = 16; o; o >>= 1) acc += __shfl_down_sync(0xffffffffu, acc, o);
@@ -77,7 +80,8 @@ __global__ void ingest_level_final(const double* __restrict__ partial, unsigned 
 }
 
 // One warp per chunk of 1024 raw samples [first_chunk, first_chunk + n_chunks).
-__global__ void __launch_bounds__(256) ingest_mask(const float2* __restrict__ iq, unsigned long long n_raw, long long first_chunk,
+template <class RAW>
+__global__ void __launch_bounds__(256) ingest_mask(const typename RAW::T* __restrict__ iq, float scale, unsigned long long n_raw, long long first_chunk,
                                                    long long n_chunks, const IngestTotals* __restrict__ tot,
                                                    unsigned int* __restrict__ mask, long long* __restrict__ chunk_last,
                                                    unsigned int* __restrict__ chunk_falls)
@@ -95,7 +99,7 @@ __global__ void __launch_bounds__(256) ingest_mask(const float2* __restrict__ iq
       const unsigned long long i = base + (unsigned)(k * 32 + lane);
       bool low = false;
       if (i < n_raw) {
-        const float2 v = __ldcs(iq + i);
+        const float2 v = RAW::cvt(RAW::ldcs(iq + i), scale);
         low = v.x * v.x + v.y * v.y < thr2;
       }
       const unsigned int b = __ballot_sync(0xffffffffu, low);
@@ -106,7 +110,7 @@ __global__ void __launch_bounds__(256) ingest_mask(const float2* __restrict__ iq
     if (lane == 0) {
       prev_top = 0;
       if (base > 0) {
-        const float2 v = iq[base - 1];
+        const float2 v = RAW::cvt(iq[base - 1], scale);
         prev_top = v.x * v.x + v.y * v.y < thr2 ? 1u : 0u;
       }
     }

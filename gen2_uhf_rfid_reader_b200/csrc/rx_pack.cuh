@@ -33,7 +33,7 @@
 //   loader      lane g streams segment g's raw samples through its two half-tile stages as warp A frees them.
 // The history is indexed by the SM (one CTA per SM: the shared-memory request guarantees it), so its size does not depend
 // on the number of segments of the launch; warp A never overwrites a sample a queued window still needs.
-// Shared memory per segment: 2 raw half-tile stages (10 KB), the last dc_length outputs of either half-tile (P1's DC
+// Shared memory per segment: 2 raw half-tile stages (10 KB; 5 KB for sc16 captures), the last dc_length outputs of either half-tile (P1's DC
 // lookback is a lane shuffle plus this tail), a pas-tile ring of |y| (1 KB per tile), the decode state of its next
 // window (112 B, static); per decoder warp C its stage (2 KB; a warp A1 in the pool uses its segment's raw stages); per CTA
 // the running-sum buffers (pas + pds x 2 per segment, 1072 B each, skewed so the chain warp's 128-bit accesses are
@@ -84,7 +84,7 @@ constexpr int kPTrig = 2;                    // windows that may open within one
 constexpr int kPackMinSmem = 116 * 1024;     // request at least this much: two CTAs never share an SM (and its history)
 
 struct PackArgs {
-  const float2* iq;
+  const void* iq;                            // raw capture (device, RAW::T[n_raw]), 16-byte aligned
   unsigned long long n_raw;
   const rfid_b200_segment* segs;
   int nseg;
@@ -103,6 +103,7 @@ struct PackArgs {
   int dstage_samples;                        // per decoder warp
   int off_dA, off_dD, off_dstage, off_seg;   // offsets from the dynamic shared-memory base
   int smem_bytes;
+  float scale;                               // sc16 captures: the int16 -> float factor (RawSc16::cvt)
 };
 
 // The decode of a segment's next window (sequence number n_decoded) between two of its phases (rx_decode.cuh: head,
@@ -198,9 +199,10 @@ __device__ __forceinline__ void pack_decode_phase(const RxConfig& C, PackWinStat
 }
 
 // PAS = pack_ring_slots(G) of the launch (PackArgs::pas): the ring indices stay compile-time divisions
-template <int DECIM, int MFQ, int PAS>
+template <int DECIM, int MFQ, int PAS, class RAW>
 __global__ void __launch_bounds__(kPackMaxThreads, 1) rx_pack_kernel(const PackArgs A)
 {
+  typedef typename RAW::T RawT;
   extern __shared__ __align__(128) unsigned char smem[];
   __shared__ PackSegCtl ctl_all[kPMaxSeg];
   __shared__ PackCtaCtl cta;
@@ -298,7 +300,7 @@ __global__ void __launch_bounds__(kPackMaxThreads, 1) rx_pack_kernel(const PackA
     const int ntiles = (n_out + kT2 - 1) / kT2;
     PackSegCtl& B = ctl_all[g];
     unsigned char* sb = smem + A.off_seg + (size_t)g * A.seg_bytes;
-    float2* raw = reinterpret_cast<float2*>(sb + A.o_raw);
+    RawT* raw = reinterpret_cast<RawT*>(sb + A.o_raw);
     float2* tail_y = reinterpret_cast<float2*>(sb + A.o_tail_y);   // [2][dc_length]: the last outputs of either half-tile
     float* ring_a = reinterpret_cast<float*>(sb + A.o_ring_a);
     float2* const y_seg = y_cta + (size_t)g * kYW;
@@ -309,7 +311,7 @@ __global__ void __launch_bounds__(kPackMaxThreads, 1) rx_pack_kernel(const PackA
 
     if (is_a) {
       // ------------------------------------------------------------------------------------- warps A0 / A1: P1 of one half-tile
-      const int odd = (int)(sg.offset & 1ull);
+      const int odd = (int)(sg.offset & (unsigned long long)(raw_granule<RAW>() - 1));   // residue of the 16-byte granule
       const float winlen_f = (float)C.win_length;
       const int h2 = ahalf;
 #ifdef RFID_B200_PHASE_PROFILE
@@ -343,7 +345,7 @@ __global__ void __launch_bounds__(kPackMaxThreads, 1) rx_pack_kernel(const PackA
         if (k * kTT < n_out) {
           const int nvalid = min(kTT, n_out - k * kTT);  // outputs of this half-tile
           const int t0 = Q * lane;
-          const float2* stage = raw + (size_t)h2 * A.raw_stage_samples;
+          const RawT* stage = raw + (size_t)h2 * A.raw_stage_samples;
           const int delta = -odd - (k > 0 ? DECIM - 1 : 0);
           const int base = DECIM * t0 - (DECIM - 1) - delta;
           // ---- block sums B(n) = x[D*n-D+1 .. D*n], ascending
@@ -352,7 +354,16 @@ __global__ void __launch_bounds__(kPackMaxThreads, 1) rx_pack_kernel(const PackA
 #pragma unroll
           for (int h = 0; h < Q; h += 2) {
             float2 x[2 * DECIM];
-            if (odd == 0 && k > 0) {
+            if constexpr (RAW::kBytes == 4) {
+              uint32_t xs[2 * DECIM];   // interior half-tiles: two outputs' raw samples, one vector run
+              if (k > 0) sc16_run(stage, base + DECIM * h, xs);
+#pragma unroll
+              for (int j = 0; j < 2 * DECIM; j++) {
+                const bool before = (k == 0) && (DECIM * (t0 + h) - (DECIM - 1) + j < 0);  // before sample 0 of the segment: +0
+                x[j] = before ? make_float2(0.f, 0.f)
+                              : RAW::cvt(k > 0 ? xs[j] : stage[base + DECIM * h + j], A.scale);
+              }
+            } else if (odd == 0 && k > 0) {
               const float4* p4 = reinterpret_cast<const float4*>(stage + base + DECIM * h);
 #pragma unroll
               for (int j = 0; j < DECIM; j++) {
@@ -386,13 +397,13 @@ __global__ void __launch_bounds__(kPackMaxThreads, 1) rx_pack_kernel(const PackA
           } else {
             // ... are the last ones of the first half-tile: lanes 0..MFQ-2 recompute them from the tail of stage 0
             mbar_wait(&B.raw_full[0], (uint32_t)(i & 1));
-            const float2* stage0 = raw;
+            const RawT* stage0 = raw;
             const int delta0 = -odd - (k - 1 > 0 ? DECIM - 1 : 0);
             const int tl = kTT - (MFQ - 1) + min(lane, MFQ - 2);          // output kTT-4 .. kTT-1 of half-tile 0
             const int b0 = DECIM * tl - (DECIM - 1) - delta0;
-            float2 hb = stage0[b0];
+            float2 hb = RAW::cvt(stage0[b0], A.scale);
 #pragma unroll
-            for (int j = 1; j < DECIM; j++) hb = c_add(hb, stage0[b0 + j]);
+            for (int j = 1; j < DECIM; j++) hb = c_add(hb, RAW::cvt(stage0[b0 + j], A.scale));
 #pragma unroll
             for (int m = 0; m < MFQ - 1; m++) halo[m] = make_float2(__shfl_sync(0xffffffffu, hb.x, m), __shfl_sync(0xffffffffu, hb.y, m));
           }
@@ -794,17 +805,18 @@ __global__ void __launch_bounds__(kPackMaxThreads, 1) rx_pack_kernel(const PackA
     const int n_out = (int)(sg.length / DECIM);
     const int nhalf = g < g_act ? (n_out + kTT - 1) / kTT : 0;
     PackSegCtl& B = ctl_all[g < G ? g : 0];
-    float2* raw = reinterpret_cast<float2*>(smem + A.off_seg + (size_t)(g < G ? g : 0) * A.seg_bytes + A.o_raw);
-    const InteriorTiles fast = interior_tiles<DECIM>(A.iq, A.n_raw, sg, nhalf);
+    RawT* raw = reinterpret_cast<RawT*>(smem + A.off_seg + (size_t)(g < G ? g : 0) * A.seg_bytes + A.o_raw);
+    const RawT* const iq = static_cast<const RawT*>(A.iq);
+    const InteriorTiles<RawT> fast = interior_tiles<DECIM, RAW>(iq, A.n_raw, sg, nhalf);
     const unsigned long long pol = l2_policy_evict_first();   // every raw sample is read exactly once
     auto issue = [&](int k) {
       const int rs_ = k & 1;
-      float2* dst = raw + (size_t)rs_ * A.raw_stage_samples;
+      RawT* dst = raw + (size_t)rs_ * A.raw_stage_samples;
       if (k >= 1 && k < fast.n) {
         mbar_arrive_expect_tx(&B.raw_full[rs_], fast.bytes);
         tma_load_1d_hint(dst, fast.src + (size_t)k * (DECIM * kTT), fast.bytes, &B.raw_full[rs_], pol);
       } else {
-        issue_tile_load<DECIM>(A.iq, A.n_raw, sg, k, dst, &B.raw_full[rs_]);
+        issue_tile_load<DECIM, RAW>(iq, A.n_raw, sg, k, dst, &B.raw_full[rs_]);
       }
     };
     for (int k = 0; k < 2 && k < nhalf; k++) issue(k);   // both stages are free at the start

@@ -149,6 +149,24 @@ RFID_B200_API int rfid_b200_decode_capture(rfid_b200_ctx* ctx, const float* d_iq
                                            rfid_b200_window_result* d_results, int32_t* d_counts,
                                            void* stream);
 
+/* Complex int16 captures (the radio's own wire format; UHD's `sc16` CPU format:
+ * n_raw complex samples, sample k = (d_iq[2k], d_iq[2k+1]) = (I, Q), 4 bytes each).
+ * Every sample is decoded as ((float)I * scale, (float)Q * scale), each component one
+ * round-to-nearest float multiply, so records, segment tables and window-tap contents
+ * equal, bit for bit, those of the fc32 entry point on that conversion of the capture.
+ * scale must be finite and > 0 (the usual choice is 1/32767, the factor UHD's host
+ * converters apply when they widen sc16 to fc32; any value works, what matters is that
+ * the same float is used wherever the two are compared).  Returns RFID_B200_EINVAL for
+ * any other scale, and for a device pointer that is not 16-byte aligned.  Segment
+ * offsets and lengths have no further alignment requirement.  The capture kernels and
+ * their choice are those of rfid_b200_decode_capture; their raw stages carry 4 bytes
+ * per sample instead of 8. */
+RFID_B200_API int rfid_b200_decode_capture_sc16(rfid_b200_ctx* ctx, const int16_t* d_iq, size_t n_raw, float scale,
+                                                const rfid_b200_segment* d_segs, int nseg,
+                                                int max_windows_per_segment,
+                                                rfid_b200_window_result* d_results, int32_t* d_counts,
+                                                void* stream);
+
 /* Same, but every pointer is a HOST pointer: copies in, decodes, copies the
  * records out, synchronises.  This is the end-to-end call a reference user makes
  * on a recorded file (apps/reader.py:102-112 in DEBUG mode). */
@@ -208,6 +226,12 @@ RFID_B200_API void rfid_b200_default_segmenter(rfid_b200_segmenter* sp);
 RFID_B200_API int rfid_b200_segment_capture(rfid_b200_ctx* ctx, const float* d_iq, size_t n_raw,
                                             const rfid_b200_segmenter* sp, rfid_b200_segment* h_segs,
                                             int capacity, int* nseg, void* stream);
+/* The same on a complex int16 capture (format, scale and argument checks as
+ * rfid_b200_decode_capture_sc16): the CW level and the low-sample mask are computed on
+ * the converted samples, so the table equals that of the fc32 conversion. */
+RFID_B200_API int rfid_b200_segment_capture_sc16(rfid_b200_ctx* ctx, const int16_t* d_iq, size_t n_raw, float scale,
+                                                 const rfid_b200_segmenter* sp, rfid_b200_segment* h_segs,
+                                                 int capacity, int* nseg, void* stream);
 
 /* File-to-records ingest, HOST pointers: uploads the capture in 16 MiB slices (pageable memory
  * through two pinned staging buffers, registered/pinned memory directly) with the threshold
@@ -218,6 +242,13 @@ RFID_B200_API int rfid_b200_ingest_capture_host(rfid_b200_ctx* ctx, const float*
                                                 const rfid_b200_segmenter* sp, int max_windows_per_segment,
                                                 rfid_b200_segment* h_segs, int seg_capacity, int* nseg,
                                                 rfid_b200_window_result* h_results, int32_t* h_counts);
+/* The same for a recorded complex int16 file (e.g. `rx_samples_to_file --type short`,
+ * `uhd_rx_cfile --output-shorts`): n_raw complex samples at h_iq, format and scale as
+ * rfid_b200_decode_capture_sc16.  The 16 MiB upload slices carry twice the samples. */
+RFID_B200_API int rfid_b200_ingest_capture_host_sc16(rfid_b200_ctx* ctx, const int16_t* h_iq, size_t n_raw, float scale,
+                                                     const rfid_b200_segmenter* sp, int max_windows_per_segment,
+                                                     rfid_b200_segment* h_segs, int seg_capacity, int* nseg,
+                                                     rfid_b200_window_result* h_results, int32_t* h_counts);
 
 /* ---------------- reader TX synthesiser + closed-loop slot simulator (SURVEY.md section 8f, rank 1) ----------------
  * The reader block's PIE command waveforms (reader_impl.cc:51-125 tables, :237-372 what every
