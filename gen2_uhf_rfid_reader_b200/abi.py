@@ -80,6 +80,21 @@ RESULT_DTYPE = np.dtype([("segment", "<i4"), ("window", "<i4"), ("open_index", "
 SEGMENT_DTYPE = np.dtype([("offset", "<u8"), ("length", "<u4"), ("reserved", "<u4")])
 assert RESULT_DTYPE.itemsize == 64 and SEGMENT_DTYPE.itemsize == 16
 
+#: kind of a reader command that is none of Query, QueryRep, ACK, NAK, QueryAdjust (its bits are still stored)
+CMD_OTHER = -1
+
+
+class CmdParams(C.Structure):
+    """rfid_b200_cmd_params (include/rfid_b200.h): reader-command decoder settings."""
+    _fields_ = [("level_frac", C.c_float), ("level_abs", C.c_float), ("gap_us", C.c_float), ("reserved", C.c_int32 * 5)]
+
+
+#: numpy view of rfid_b200_command (64 bytes)
+COMMAND_DTYPE = np.dtype([("segment", "<i4"), ("index", "<i4"), ("start", "<i4"), ("end", "<i4"), ("kind", "<i4"),
+                          ("n_bits", "<i4"), ("tari", "<i4"), ("rtcal", "<i4"), ("trcal", "<i4"), ("crc_ok", "<i4"),
+                          ("arg", "<i4"), ("reserved", "<i4"), ("bits", "u1", (16,))])
+assert COMMAND_DTYPE.itemsize == 64 and C.sizeof(CmdParams) == 32
+
 
 def make_segments(offsets, lengths):
     segs = np.zeros(len(offsets), dtype=SEGMENT_DTYPE)

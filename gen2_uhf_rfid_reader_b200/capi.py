@@ -98,6 +98,15 @@ def load_library():
     L.rfid_b200_sim_segment_length.argtypes = [vp, C.POINTER(abi.SimParams)]
     L.rfid_b200_sim_capture.restype = C.c_int
     L.rfid_b200_sim_capture.argtypes = [vp, C.POINTER(abi.SimParams), C.c_int64, C.c_int, vp, vp, vp, vp]
+    L.rfid_b200_default_cmd_params.argtypes = [C.POINTER(abi.CmdParams)]
+    L.rfid_b200_decode_commands.restype = C.c_int
+    L.rfid_b200_decode_commands.argtypes = [vp, vp, C.c_size_t, vp, C.c_int, C.POINTER(abi.CmdParams), C.c_int, vp, vp, vp]
+    L.rfid_b200_decode_commands_sc16.restype = C.c_int
+    L.rfid_b200_decode_commands_sc16.argtypes = [vp, vp, C.c_size_t, C.c_float, vp, C.c_int, C.POINTER(abi.CmdParams),
+                                                 C.c_int, vp, vp, vp]
+    L.rfid_b200_decode_commands_host.restype = C.c_int
+    L.rfid_b200_decode_commands_host.argtypes = [vp, vp, C.c_size_t, vp, C.c_int, C.POINTER(abi.CmdParams), C.c_int, vp,
+                                                 vp]
     _lib = L
     return L
 
@@ -111,6 +120,8 @@ EXPORTED_SYMBOLS = [
     "rfid_b200_default_segmenter", "rfid_b200_segment_capture", "rfid_b200_ingest_capture_host",
     "rfid_b200_tx_synth", "rfid_b200_default_sim", "rfid_b200_sim_segment_length", "rfid_b200_sim_capture",
     "rfid_b200_decode_capture_sc16", "rfid_b200_segment_capture_sc16", "rfid_b200_ingest_capture_host_sc16",
+    "rfid_b200_default_cmd_params", "rfid_b200_decode_commands", "rfid_b200_decode_commands_sc16",
+    "rfid_b200_decode_commands_host",
 ]
 
 
@@ -137,6 +148,15 @@ def default_segmenter(**kw):
     for k, v in kw.items():
         setattr(sp, k, type(getattr(sp, k))(v))
     return sp
+
+
+def default_cmd_params(**kw):
+    """rfid_b200_cmd_params with the library's defaults (level_frac 0.5, level_abs 0, gap_us 400), fields set by kw."""
+    cp = abi.CmdParams()
+    load_library().rfid_b200_default_cmd_params(C.byref(cp))
+    for k, v in kw.items():
+        setattr(cp, k, type(getattr(cp, k))(v))
+    return cp
 
 
 def default_params(**kw):
@@ -224,6 +244,49 @@ class Gen2Rx:
         """Same call on raw (e.g. pinned) host pointers: no Python-side copies."""
         rc = self.lib.rfid_b200_decode_capture_host(self.h, iq_ptr, n_raw, segs_ptr, nseg, max_windows, res_ptr, cnt_ptr)
         self._ck(rc, "rfid_b200_decode_capture_host")
+
+    # ---------------------------------------------------------------- capture mode: the reader's commands
+    def decode_commands(self, iq, segs, max_commands=8, commands=None, counts=None, stream=None, scale=SC16_SCALE,
+                        params=None):
+        """The reader's PIE commands in every segment (rule: include/rfid_b200.h).  iq and segs as in `decode_capture`
+        (complex64 / float32 interleaved, or an sc16 torch.int16 tensor decoded as its conversion); params: `CmdParams`
+        (None: defaults, see `default_cmd_params`).  Asynchronous on `stream`.  Returns (commands uint8[nseg*max,64],
+        counts int32[nseg]); `commands_to_numpy` views them as COMMAND_DTYPE."""
+        import torch
+        nseg = segs.numel() * segs.element_size() // 16
+        sc16 = iq.dtype == torch.int16
+        n_raw = _sc16_samples(iq) if sc16 else (iq.numel() if iq.is_complex() else iq.numel() // 2)
+        if commands is None:
+            commands = torch.zeros((nseg * max_commands, 64), dtype=torch.uint8, device=iq.device)
+        if counts is None:
+            counts = torch.zeros(nseg, dtype=torch.int32, device=iq.device)
+        s = stream if stream is not None else torch.cuda.current_stream(iq.device)
+        cp = C.byref(params) if params is not None else None
+        if sc16:
+            rc = self.lib.rfid_b200_decode_commands_sc16(self.h, iq.data_ptr(), n_raw, scale, segs.data_ptr(), nseg, cp,
+                                                         max_commands, commands.data_ptr(), counts.data_ptr(),
+                                                         s.cuda_stream)
+            self._ck(rc, "rfid_b200_decode_commands_sc16")
+        else:
+            rc = self.lib.rfid_b200_decode_commands(self.h, iq.data_ptr(), n_raw, segs.data_ptr(), nseg, cp, max_commands,
+                                                    commands.data_ptr(), counts.data_ptr(), s.cuda_stream)
+            self._ck(rc, "rfid_b200_decode_commands")
+        return commands, counts
+
+    def decode_commands_host(self, iq, segs, max_commands=8, params=None):
+        """Host arrays in, host records out: iq complex64 ndarray, segs SEGMENT_DTYPE -> (COMMAND_DTYPE[nseg, max],
+        int32[nseg])."""
+        raw = np.ascontiguousarray(iq).view(np.float32).ravel()
+        segs = np.ascontiguousarray(segs, dtype=abi.SEGMENT_DTYPE)
+        nseg = segs.size
+        cmds = np.zeros((nseg, max_commands), dtype=abi.COMMAND_DTYPE)
+        counts = np.zeros(nseg, dtype=np.int32)
+        cp = C.byref(params) if params is not None else None
+        rc = self.lib.rfid_b200_decode_commands_host(self.h, raw.ctypes.data, raw.size // 2, segs.ctypes.data, nseg, cp,
+                                                     max_commands, cmds.ctypes.data if cmds.size else None,
+                                                     counts.ctypes.data)
+        self._ck(rc, "rfid_b200_decode_commands_host")
+        return cmds, counts
 
     # ---------------------------------------------------------------- capture ingest
     def segment_capture(self, iq, segmenter=None, capacity=None, stream=None, scale=SC16_SCALE):
@@ -378,3 +441,58 @@ def results_to_numpy(results, counts, max_windows):
     r = results.cpu().numpy().reshape(-1).view(abi.RESULT_DTYPE)
     c = counts.cpu().numpy()
     return r.reshape(c.size, max_windows), c
+
+
+def commands_to_numpy(cmds, counts, max_commands):
+    """device uint8[nseg*max_commands,64] + int32[nseg] -> (COMMAND_DTYPE[nseg,max_commands], int32[nseg])"""
+    r = cmds.cpu().numpy().reshape(-1).view(abi.COMMAND_DTYPE)
+    c = counts.cpu().numpy()
+    return r.reshape(c.size, max_commands), c
+
+
+#: one row per stored tag window: the reader command that armed it (see `transcript`)
+TRANSCRIPT_DTYPE = np.dtype([("segment", "<i4"), ("window", "<i4"), ("kind", "<i4"), ("command", "<i4"),
+                             ("cmd_kind", "<i4"), ("cmd_arg", "<i4"), ("ack_echo", "<i4"), ("turnaround_us", "<f8")])
+
+
+def transcript(cmds, cmd_counts, recs, counts, decim=5, adc_rate=2_000_000):
+    """Pair every stored tag window with the reader command that armed it (host numpy only).
+
+    cmds, cmd_counts: `decode_commands` output (COMMAND_DTYPE[nseg, max_commands]); recs, counts: `decode_capture` output
+    (RESULT_DTYPE[nseg, max_windows]) of the same segment table.  Per window:
+      command        index of the last stored command of the segment with end <= open_index*decim (raw samples), or -1;
+      cmd_kind/arg   that command's kind and arg (-1 without one);
+      ack_echo       EPC windows: 1 if the arming command is an ACK whose arg equals the tag_id of the segment's preceding
+                     RN16 window, else 0; RN16 windows: -1;
+      turnaround_us  EPC windows armed by an ACK that follows an RN16 window: from the RN16 window's end,
+                     (open_index + length)*decim, to the ACK's start, in microseconds at adc_rate; NaN otherwise.
+    """
+    cmds = np.asarray(cmds, dtype=abi.COMMAND_DTYPE)
+    recs = np.asarray(recs, dtype=abi.RESULT_DTYPE)
+    cmd_counts = np.asarray(cmd_counts)
+    counts = np.asarray(counts)
+    rows = []
+    for s in range(counts.size):
+        cs = cmds[s, :max(0, min(int(cmd_counts[s]), cmds.shape[1]))]
+        ends = cs["end"].astype(np.int64)
+        prev_rn16 = None
+        for w in recs[s, :max(0, min(int(counts[s]), recs.shape[1]))]:
+            r = np.zeros((), dtype=TRANSCRIPT_DTYPE)
+            r["segment"], r["window"], r["kind"] = s, w["window"], w["kind"]
+            k = int(np.searchsorted(ends, int(w["open_index"]) * decim, side="right")) - 1 if cs.size else -1
+            # (ends are increasing: commands do not overlap)
+            r["command"] = k
+            r["cmd_kind"] = cs["kind"][k] if k >= 0 else -1
+            r["cmd_arg"] = cs["arg"][k] if k >= 0 else -1
+            r["ack_echo"] = -1
+            r["turnaround_us"] = np.nan
+            if int(w["kind"]) == abi.EPC:
+                is_ack = k >= 0 and int(cs["kind"][k]) == abi.TX_ACK
+                r["ack_echo"] = int(is_ack and prev_rn16 is not None and int(cs["arg"][k]) == int(prev_rn16["tag_id"]))
+                if is_ack and prev_rn16 is not None:
+                    rn16_end = (int(prev_rn16["open_index"]) + int(prev_rn16["length"])) * decim
+                    r["turnaround_us"] = (int(cs["start"][k]) - rn16_end) * 1e6 / adc_rate
+            else:
+                prev_rn16 = w
+            rows.append(r)
+    return np.array(rows, dtype=TRANSCRIPT_DTYPE)

@@ -13,6 +13,7 @@
 #include <vector>
 
 #include "rx_block.cuh"
+#include "rx_cmd.cuh"
 #include "rx_common.cuh"
 #include "rx_fused.cuh"
 #include "rx_fused_split.cuh"
@@ -76,6 +77,8 @@ struct rfid_b200_ctx {
   void* d_script; size_t d_script_bytes;
   void* d_sim_res; size_t d_sim_res_bytes;
   void* d_sim_cnt; size_t d_sim_cnt_bytes;
+  // host-mode command records
+  void* d_cmd; size_t d_cmd_bytes;
 };
 
 namespace {
@@ -406,6 +409,7 @@ int rfid_b200_create(const rfid_b200_params* p, rfid_b200_ctx** out)
   ctx->d_mask_bytes = ctx->d_chunk_bytes = ctx->d_bursts_bytes = 0;
   ctx->d_script = ctx->d_sim_res = ctx->d_sim_cnt = nullptr;
   ctx->d_script_bytes = ctx->d_sim_res_bytes = ctx->d_sim_cnt_bytes = 0;
+  ctx->d_cmd = nullptr; ctx->d_cmd_bytes = 0;
   ctx->h_stage[0] = ctx->h_stage[1] = nullptr; ctx->ev_stage[0] = ctx->ev_stage[1] = nullptr;
   memset(&ctx->layout, 0, sizeof(ctx->layout));
   memset(&ctx->layout_sc16, 0, sizeof(ctx->layout_sc16));
@@ -494,7 +498,7 @@ void rfid_b200_destroy(rfid_b200_ctx* ctx)
   if (ctx->h_blk) cudaFreeHost(ctx->h_blk);
   void* ptrs[] = {ctx->d_blk, ctx->d_win, ctx->d_yhist, ctx->d_iq, ctx->d_segs, ctx->d_res, ctx->d_cnt, ctx->d_in, ctx->d_out, ctx->d_m2, ctx->d_mf,
                   ctx->d_gate, ctx->d_gate_out, ctx->d_one, ctx->d_mask, ctx->d_chunk, ctx->d_bursts, ctx->d_ing,
-                  ctx->d_script, ctx->d_sim_res, ctx->d_sim_cnt};
+                  ctx->d_script, ctx->d_sim_res, ctx->d_sim_cnt, ctx->d_cmd};
   for (void* p : ptrs)
     if (p) cudaFree(p);
   for (int b = 0; b < 2; b++) {
@@ -1250,6 +1254,99 @@ int rfid_b200_sim_capture(rfid_b200_ctx* ctx, const rfid_b200_sim_params* p, int
     launches = 3;
   }
   ctx->last_launches = launches;
+  return RFID_B200_OK;
+}
+
+// ------------------------------------------------------------------ capture mode: the reader's commands
+void rfid_b200_default_cmd_params(rfid_b200_cmd_params* cp)
+{
+  if (!cp) return;
+  memset(cp, 0, sizeof(*cp));
+  cp->level_frac = 0.5f;   // the segmenter's
+  cp->gap_us = 400.f;
+  cp->level_abs = 0.f;
+}
+
+// the kernel's settings from the caller's (NULL = defaults); RFID_B200_EINVAL when they are out of range
+static int resolve_cmd_params(const rfid_b200_ctx* ctx, const rfid_b200_cmd_params* cp, CmdArgs& A)
+{
+  rfid_b200_cmd_params d;
+  rfid_b200_default_cmd_params(&d);
+  if (cp) d = *cp;
+  if (!(d.level_frac > 0.f && d.level_frac < 1.f) || !(d.level_abs >= 0.f) || !std::isfinite(d.level_abs) || !(d.gap_us > 0.f))
+    return RFID_B200_EINVAL;
+  A.frac2 = d.level_frac * d.level_frac;
+  A.use_abs = d.level_abs > 0.f;
+  A.abs2 = d.level_abs * d.level_abs;
+  const double gap = (double)d.gap_us * 1e-6 * ctx->cfg.adc_rate;   // (a gap beyond any segment length acts as INT32_MAX)
+  A.gap = gap >= 2147483647.0 ? 2147483647 : (int)gap;
+  return RFID_B200_OK;
+}
+
+static int decode_commands_impl(rfid_b200_ctx* ctx, const void* d_iq, bool sc16, float scale, size_t n_raw,
+                                const rfid_b200_segment* d_segs, int nseg, const rfid_b200_cmd_params* cp, int max_cmds,
+                                rfid_b200_command* d_cmds, int32_t* d_counts, void* stream)
+{
+  if (!ctx || !d_iq || !d_segs || !d_counts || nseg < 0 || max_cmds < 0 || (max_cmds > 0 && !d_cmds)) return RFID_B200_EINVAL;
+  if ((reinterpret_cast<uintptr_t>(d_iq) & (sc16 ? 15u : 7u)) != 0) return RFID_B200_EINVAL;
+  CmdArgs A;
+  int rc = resolve_cmd_params(ctx, cp, A);
+  if (rc) return rc;
+  if (nseg == 0) return RFID_B200_OK;
+  CK(cudaSetDevice(ctx->device));
+  A.iq = d_iq; A.scale = scale; A.n_raw = n_raw; A.segs = d_segs; A.nseg = nseg; A.max_cmds = max_cmds;
+  A.cmds = d_cmds; A.counts = d_counts;
+  cudaStream_t s = (cudaStream_t)stream;
+  if (sc16) rx_cmd_kernel<RawSc16><<<nseg, kCmdThreads, 0, s>>>(A);
+  else rx_cmd_kernel<RawFc32><<<nseg, kCmdThreads, 0, s>>>(A);
+  CK(cudaGetLastError());
+  return RFID_B200_OK;
+}
+
+int rfid_b200_decode_commands(rfid_b200_ctx* ctx, const float* d_iq, size_t n_raw, const rfid_b200_segment* d_segs, int nseg,
+                              const rfid_b200_cmd_params* cp, int max_commands_per_segment, rfid_b200_command* d_cmds,
+                              int32_t* d_counts, void* stream)
+{
+  return decode_commands_impl(ctx, d_iq, false, 1.f, n_raw, d_segs, nseg, cp, max_commands_per_segment, d_cmds, d_counts, stream);
+}
+
+int rfid_b200_decode_commands_sc16(rfid_b200_ctx* ctx, const int16_t* d_iq, size_t n_raw, float scale,
+                                   const rfid_b200_segment* d_segs, int nseg, const rfid_b200_cmd_params* cp,
+                                   int max_commands_per_segment, rfid_b200_command* d_cmds, int32_t* d_counts, void* stream)
+{
+  if (!scale_ok(scale)) return RFID_B200_EINVAL;
+  return decode_commands_impl(ctx, d_iq, true, scale, n_raw, d_segs, nseg, cp, max_commands_per_segment, d_cmds, d_counts, stream);
+}
+
+int rfid_b200_decode_commands_host(rfid_b200_ctx* ctx, const float* h_iq, size_t n_raw, const rfid_b200_segment* h_segs, int nseg,
+                                   const rfid_b200_cmd_params* cp, int max_commands_per_segment, rfid_b200_command* h_cmds,
+                                   int32_t* h_counts)
+{
+  if (!ctx || !h_iq || !h_segs || !h_counts || nseg < 0 || max_commands_per_segment < 0 ||
+      (max_commands_per_segment > 0 && !h_cmds))
+    return RFID_B200_EINVAL;
+  CmdArgs A;
+  int rc = resolve_cmd_params(ctx, cp, A);
+  if (rc) return rc;
+  for (int i = 0; i < nseg; i++)
+    if (h_segs[i].length > 0x7fffffffu) return RFID_B200_EINVAL;
+  if (nseg == 0) return RFID_B200_OK;
+  CK(cudaSetDevice(ctx->device));
+  const size_t cmd_bytes = (size_t)nseg * max_commands_per_segment * sizeof(rfid_b200_command);
+  if ((rc = grow(ctx, &ctx->d_iq, &ctx->d_iq_bytes, n_raw * 8 + 16))) return rc;
+  if ((rc = grow(ctx, &ctx->d_segs, &ctx->d_segs_bytes, (size_t)nseg * sizeof(rfid_b200_segment)))) return rc;
+  if ((rc = grow(ctx, &ctx->d_cmd, &ctx->d_cmd_bytes, cmd_bytes))) return rc;
+  if ((rc = grow(ctx, &ctx->d_cnt, &ctx->d_cnt_bytes, (size_t)nseg * 4))) return rc;
+  cudaStream_t s = ctx->stream;
+  CK(cudaMemcpyAsync(ctx->d_iq, h_iq, n_raw * 8, cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(ctx->d_segs, h_segs, (size_t)nseg * sizeof(rfid_b200_segment), cudaMemcpyHostToDevice, s));
+  if (cmd_bytes) CK(cudaMemsetAsync(ctx->d_cmd, 0, cmd_bytes, s));
+  rc = decode_commands_impl(ctx, ctx->d_iq, false, 1.f, n_raw, (const rfid_b200_segment*)ctx->d_segs, nseg, cp,
+                            max_commands_per_segment, (rfid_b200_command*)ctx->d_cmd, (int32_t*)ctx->d_cnt, s);
+  if (rc) return rc;
+  if (cmd_bytes) CK(cudaMemcpyAsync(h_cmds, ctx->d_cmd, cmd_bytes, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(h_counts, ctx->d_cnt, (size_t)nseg * 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
   return RFID_B200_OK;
 }
 

@@ -320,6 +320,78 @@ RFID_B200_API int rfid_b200_sim_capture(rfid_b200_ctx* ctx, const rfid_b200_sim_
                                         int nseg, float* d_iq, rfid_b200_segment* d_segs,
                                         rfid_b200_sim_truth* d_truth, void* stream);
 
+/* ---------------- capture mode: the reader's commands ----------------
+ * In a monostatic capture the reader's TX leaks into the RX at full carrier level, so every segment holds the reader's
+ * PIE commands (reader_impl.cc:51-125,251-372) besides the tag's replies.  rfid_b200_decode_commands reads them back, per
+ * segment and independently of every other segment and of the capture outside it (so the result does not depend on how a
+ * capture is sharded):
+ *   - p[i] = re*re + im*im of the (converted) sample, in float with each operation rounded;
+ *   - thr2 = (level_frac*level_frac) * P, P = max p over the segment (NaN samples ignored); level_abs > 0 gives
+ *     thr2 = level_abs*level_abs instead, for captures with outliers above 1/level_frac of the carrier amplitude.
+ *     Sample i is low iff p[i] < thr2;
+ *   - a fall is a low sample whose predecessor inside the segment is high (a low first sample is a fall);
+ *   - a burst starts at a fall that has no low sample before it in the segment, or whose previous low sample prev
+ *     satisfies fall - prev - 1 >= gap, gap = (int)(gap_us * 1e-6 * adc_rate) raw samples (the segmenter's test);
+ *   - bursts of fewer than 4 falls are not reported.  Of the others, with d_k the fall-to-fall intervals: tari = d_0,
+ *     rtcal = d_1; d_2 > rtcal means a preamble (trcal = d_2, data from d_3), otherwise a frame-sync (trcal = 0, data
+ *     from d_2); every data interval is one bit, 1 iff 2*d > rtcal (every PIE symbol ends with its pulse);
+ *   - start = the burst's first fall, end = the sample after its last low sample (or the segment length): raw samples
+ *     relative to the segment;
+ *   - kind (sync, bits, prefix -> arg, crc_ok):
+ *       RFID_B200_TX_QUERY         preamble   22  1000      Q (bits 13-16), CRC-5 of bits 0-16 = bits 17-21 ? 1 : 0
+ *       RFID_B200_TX_QUERY_REP     frame-sync  4  00        session (bits 2-3), -1
+ *       RFID_B200_TX_ACK           frame-sync 18  01        RN16 (bits 2-17), -1
+ *       RFID_B200_TX_QUERY_ADJUST  frame-sync  9  1001      session (bits 4-5), -1
+ *       RFID_B200_TX_NAK           frame-sync  8  11000000  -1, -1
+ *     anything else is RFID_B200_CMD_OTHER (arg and crc_ok -1) with its bits stored.
+ * Inside a command the longest high stretch is TRcal - PW (188 us); between the commands of an inventory lies a tag
+ * reply.  The reference's NAK is followed by only CW_D = 250 us of carrier (reader_impl.cc:233-249), so at the default
+ * gap of 400 us a NAK and the command after it form one burst, reported as OTHER; a gap_us between about 190 and 249
+ * separates them. */
+#define RFID_B200_CMD_OTHER (-1)
+
+typedef struct rfid_b200_cmd_params {
+  float level_frac;    /* in (0, 1); 0.5 */
+  float level_abs;     /* >= 0, finite; 0 = use level_frac */
+  float gap_us;        /* > 0; 400 */
+  int32_t reserved[5];
+} rfid_b200_cmd_params;
+
+typedef struct rfid_b200_command { /* 64 bytes */
+  int32_t segment, index;         /* segment-table index; ordinal inside the segment */
+  int32_t start, end;             /* raw samples, segment relative (rule above) */
+  int32_t kind, n_bits;           /* RFID_B200_TX_* / RFID_B200_CMD_OTHER; all data bits (> 128: the first 128 stored) */
+  int32_t tari, rtcal, trcal;     /* raw samples; trcal 0 = frame-sync */
+  int32_t crc_ok, arg, reserved;
+  uint8_t bits[16];               /* data bits, MSB first */
+} rfid_b200_command;
+
+RFID_B200_API void rfid_b200_default_cmd_params(rfid_b200_cmd_params* cp);
+
+/* Commands of nseg segments of a capture resident in device memory (fc32; d_iq 8-byte aligned), asynchronously on
+ * `stream`, conventions of rfid_b200_decode_capture: command k of segment s goes to d_cmds[s*max_commands_per_segment+k],
+ * d_counts[s] receives the number of commands found (those beyond max_commands_per_segment are counted, not stored;
+ * max_commands_per_segment may be 0, and d_cmds NULL with it).  A segment is cut at the end of the capture.  A segment
+ * longer than INT32_MAX samples gets d_counts[s] = RFID_B200_EINVAL and no records.  cp NULL = defaults.  Returns
+ * RFID_B200_EINVAL for level_frac outside (0, 1), a negative or non-finite level_abs, gap_us <= 0 and negative counts.
+ * One CTA per segment reads the segment twice (peak, then masks). */
+RFID_B200_API int rfid_b200_decode_commands(rfid_b200_ctx* ctx, const float* d_iq, size_t n_raw,
+                                            const rfid_b200_segment* d_segs, int nseg, const rfid_b200_cmd_params* cp,
+                                            int max_commands_per_segment, rfid_b200_command* d_cmds, int32_t* d_counts,
+                                            void* stream);
+/* The same on a complex int16 capture (format, scale and argument checks as rfid_b200_decode_capture_sc16): the records
+ * equal those of the fc32 conversion. */
+RFID_B200_API int rfid_b200_decode_commands_sc16(rfid_b200_ctx* ctx, const int16_t* d_iq, size_t n_raw, float scale,
+                                                 const rfid_b200_segment* d_segs, int nseg, const rfid_b200_cmd_params* cp,
+                                                 int max_commands_per_segment, rfid_b200_command* d_cmds,
+                                                 int32_t* d_counts, void* stream);
+/* HOST pointers (fc32): copies in, decodes, copies the records out, synchronises.  A segment longer than INT32_MAX
+ * samples is RFID_B200_EINVAL. */
+RFID_B200_API int rfid_b200_decode_commands_host(rfid_b200_ctx* ctx, const float* h_iq, size_t n_raw,
+                                                 const rfid_b200_segment* h_segs, int nseg, const rfid_b200_cmd_params* cp,
+                                                 int max_commands_per_segment, rfid_b200_command* h_cmds,
+                                                 int32_t* h_counts);
+
 /* ---------------- block mode (GNU Radio drop-in) ----------------
  * Called from the thin host blocks' general_work(); HOST pointers, owned by the
  * scheduler, touched only during the call.  State lives in the context (device
