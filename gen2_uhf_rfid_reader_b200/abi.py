@@ -96,6 +96,23 @@ COMMAND_DTYPE = np.dtype([("segment", "<i4"), ("index", "<i4"), ("start", "<i4")
 assert COMMAND_DTYPE.itemsize == 64 and C.sizeof(CmdParams) == 32
 
 
+SLOT_EMPTY, SLOT_SINGLE, SLOT_COLLISION = 0, 1, 2
+
+
+class QualityParams(C.Structure):
+    """rfid_b200_quality_params (include/rfid_b200.h): slot-outcome thresholds in dB."""
+    _fields_ = [("empty_db", C.c_float), ("single_snr_db", C.c_float), ("reserved", C.c_int32 * 6)]
+
+
+class Quality(C.Structure):
+    _fields_ = [("energy", C.c_float), ("snr", C.c_float), ("outcome", C.c_int32), ("n_decisions", C.c_int32)]
+
+
+#: numpy view of rfid_b200_quality (16 bytes): linear reply-energy and decision-SNR ratios, RFID_B200_SLOT_* outcome
+QUALITY_DTYPE = np.dtype([("energy", "<f4"), ("snr", "<f4"), ("outcome", "<i4"), ("n_decisions", "<i4")])
+assert QUALITY_DTYPE.itemsize == C.sizeof(Quality) == 16 and C.sizeof(QualityParams) == 32
+
+
 def make_segments(offsets, lengths):
     segs = np.zeros(len(offsets), dtype=SEGMENT_DTYPE)
     segs["offset"] = np.asarray(offsets, dtype=np.uint64)

@@ -107,6 +107,9 @@ def load_library():
     L.rfid_b200_decode_commands_host.restype = C.c_int
     L.rfid_b200_decode_commands_host.argtypes = [vp, vp, C.c_size_t, vp, C.c_int, C.POINTER(abi.CmdParams), C.c_int, vp,
                                                  vp]
+    L.rfid_b200_default_quality_params.argtypes = [C.POINTER(abi.QualityParams)]
+    L.rfid_b200_window_quality.restype = C.c_int
+    L.rfid_b200_window_quality.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.POINTER(abi.QualityParams), vp, vp]
     _lib = L
     return L
 
@@ -121,7 +124,7 @@ EXPORTED_SYMBOLS = [
     "rfid_b200_tx_synth", "rfid_b200_default_sim", "rfid_b200_sim_segment_length", "rfid_b200_sim_capture",
     "rfid_b200_decode_capture_sc16", "rfid_b200_segment_capture_sc16", "rfid_b200_ingest_capture_host_sc16",
     "rfid_b200_default_cmd_params", "rfid_b200_decode_commands", "rfid_b200_decode_commands_sc16",
-    "rfid_b200_decode_commands_host",
+    "rfid_b200_decode_commands_host", "rfid_b200_default_quality_params", "rfid_b200_window_quality",
 ]
 
 
@@ -157,6 +160,15 @@ def default_cmd_params(**kw):
     for k, v in kw.items():
         setattr(cp, k, type(getattr(cp, k))(v))
     return cp
+
+
+def default_quality_params(**kw):
+    """rfid_b200_quality_params with the library's defaults (empty_db 9.5, single_snr_db 8.8), fields set by kw."""
+    qp = abi.QualityParams()
+    load_library().rfid_b200_default_quality_params(C.byref(qp))
+    for k, v in kw.items():
+        setattr(qp, k, type(getattr(qp, k))(v))
+    return qp
 
 
 def default_params(**kw):
@@ -287,6 +299,43 @@ class Gen2Rx:
                                                      counts.ctypes.data)
         self._ck(rc, "rfid_b200_decode_commands_host")
         return cmds, counts
+
+    # ---------------------------------------------------------------- capture mode: reply quality and slot outcome
+    def window_quality(self, windows, results, counts, max_windows, params=None, quality=None, stream=None):
+        """Quality records (rule: include/rfid_b200.h) of the stored windows of a `decode_capture` call: windows = the
+        window tap it wrote (CUDA complex64 / float32 tensor of nseg * max_windows * len_epc samples), results / counts
+        its outputs; params: `QualityParams` (None: defaults, see `default_quality_params`).  Asynchronous on `stream`.
+        Returns quality, a CUDA uint8 tensor [nseg * max_windows, 16] (`quality_to_numpy` views it as QUALITY_DTYPE);
+        slots beyond a segment's stored records are left as they were (zero when allocated here)."""
+        import torch
+        nseg = counts.numel()
+        if windows.numel() * windows.element_size() < nseg * max_windows * self.len_epc * 8:
+            raise ValueError("the window tap holds fewer than nseg * max_windows * len_epc complex samples")
+        if quality is None:
+            quality = torch.zeros((nseg * max_windows, 16), dtype=torch.uint8, device=results.device)
+        s = stream if stream is not None else torch.cuda.current_stream(results.device)
+        qp = C.byref(params) if params is not None else None
+        rc = self.lib.rfid_b200_window_quality(self.h, windows.data_ptr(), results.data_ptr(), counts.data_ptr(), nseg,
+                                               max_windows, qp, quality.data_ptr(), s.cuda_stream)
+        self._ck(rc, "rfid_b200_window_quality")
+        return quality
+
+    def decode_capture_quality(self, iq, segs, max_windows=2, params=None, scale=SC16_SCALE):
+        """`decode_capture` with the window tap set for this one call, then `window_quality` on what it wrote.  iq, segs
+        and scale as in `decode_capture` (fc32 or sc16).  The tap takes nseg * max_windows * len_epc * 8 bytes of
+        device memory (3.5 GB for 160,000 segments of 2 windows at 2 MS/s); it is released to torch's stream-ordered
+        allocator on return, so the call stays asynchronous on the current stream like `decode_capture`.  Returns
+        (results, counts, quality) as device tensors."""
+        import torch
+        nseg = segs.numel() * segs.element_size() // 16
+        tap = torch.empty(nseg * max_windows * self.len_epc, dtype=torch.complex64, device=iq.device)
+        self.set_window_tap(tap)
+        try:
+            results, counts = self.decode_capture(iq, segs, max_windows=max_windows, scale=scale)
+            quality = self.window_quality(tap, results, counts, max_windows, params=params)
+        finally:
+            self.set_window_tap(None)
+        return results, counts, quality
 
     # ---------------------------------------------------------------- capture ingest
     def segment_capture(self, iq, segmenter=None, capacity=None, stream=None, scale=SC16_SCALE):
@@ -496,3 +545,61 @@ def transcript(cmds, cmd_counts, recs, counts, decim=5, adc_rate=2_000_000):
                 prev_rn16 = w
             rows.append(r)
     return np.array(rows, dtype=TRANSCRIPT_DTYPE)
+
+
+def quality_to_numpy(quality, counts, max_windows):
+    """device uint8[nseg*max_windows,16] + int32[nseg] -> (QUALITY_DTYPE[nseg,max_windows], int32[nseg])"""
+    q = quality.cpu().numpy().reshape(-1).view(abi.QUALITY_DTYPE)
+    c = counts.cpu().numpy()
+    return q.reshape(c.size, max_windows), c
+
+
+#: one row per segment: what its RN16 and EPC windows say about the slot (see `slot_table`)
+SLOT_DTYPE = np.dtype([("segment", "<i4"), ("rn16_outcome", "<i4"), ("epc_outcome", "<i4"), ("tag_id", "<i4"),
+                       ("crc_ok", "<i4"), ("rn16_energy_db", "<f8"), ("rn16_snr_db", "<f8"), ("epc_energy_db", "<f8"),
+                       ("epc_snr_db", "<f8")])
+
+
+def _db(x):
+    with np.errstate(divide="ignore", invalid="ignore"):
+        return 10.0 * np.log10(np.float64(x))
+
+
+def slot_table(recs, counts, quality):
+    """One row per segment of a capture decoded one slot per segment (host numpy only).  recs, counts: `decode_capture`
+    output (RESULT_DTYPE[nseg, max_windows]); quality: `window_quality` output (QUALITY_DTYPE[nseg, max_windows]).  The
+    slot's RN16 window is the segment's first stored window, its EPC window the second.  Outcomes are RFID_B200_SLOT_*
+    or -1 where the segment has no such window; tag_id and crc_ok come from the EPC record (-1 without one); energy and
+    SNR in dB (NaN without a window)."""
+    recs = np.asarray(recs, dtype=abi.RESULT_DTYPE)
+    quality = np.asarray(quality, dtype=abi.QUALITY_DTYPE)
+    counts = np.asarray(counts)
+    out = np.zeros(counts.size, dtype=SLOT_DTYPE)
+    out["segment"] = np.arange(counts.size)
+    for f in ("rn16_outcome", "epc_outcome", "tag_id", "crc_ok"):
+        out[f] = -1
+    for f in ("rn16_energy_db", "rn16_snr_db", "epc_energy_db", "epc_snr_db"):
+        out[f] = np.nan
+    n = np.minimum(np.maximum(counts, 0), recs.shape[1])
+    for k, name in ((0, "rn16"), (1, "epc")):
+        has = n > k
+        if k >= recs.shape[1] or not has.any():
+            continue
+        q = quality[has, k]
+        out[name + "_outcome"][has] = q["outcome"]
+        out[name + "_energy_db"][has] = _db(q["energy"])
+        out[name + "_snr_db"][has] = _db(q["snr"])
+        if name == "epc":
+            out["tag_id"][has] = recs[has, k]["tag_id"]
+            out["crc_ok"][has] = recs[has, k]["crc_ok"]
+    return out
+
+
+def inventory_summary(recs, counts, quality):
+    """Counts of an inventory's slots from `slot_table`: empty, single and collided slots (RN16 outcome; segments
+    without an RN16 window are not counted), and the single slots whose EPC passed its CRC."""
+    t = slot_table(recs, counts, quality)
+    rn = t["rn16_outcome"]
+    return {"slots": int((rn >= 0).sum()), "empty": int((rn == abi.SLOT_EMPTY).sum()),
+            "single": int((rn == abi.SLOT_SINGLE).sum()), "collision": int((rn == abi.SLOT_COLLISION).sum()),
+            "single_epc_ok": int(((rn == abi.SLOT_SINGLE) & (t["crc_ok"] == 1)).sum())}

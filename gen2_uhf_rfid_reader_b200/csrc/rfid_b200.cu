@@ -19,6 +19,7 @@
 #include "rx_fused_split.cuh"
 #include "rx_ingest.cuh"
 #include "rx_pack.cuh"
+#include "rx_quality.cuh"
 #include "tx_synth.cuh"
 
 using namespace rfid_b200;
@@ -1347,6 +1348,41 @@ int rfid_b200_decode_commands_host(rfid_b200_ctx* ctx, const float* h_iq, size_t
   if (cmd_bytes) CK(cudaMemcpyAsync(h_cmds, ctx->d_cmd, cmd_bytes, cudaMemcpyDeviceToHost, s));
   CK(cudaMemcpyAsync(h_counts, ctx->d_cnt, (size_t)nseg * 4, cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
+  return RFID_B200_OK;
+}
+
+// ------------------------------------------------------------------ capture mode: reply quality and slot outcome
+void rfid_b200_default_quality_params(rfid_b200_quality_params* qp)
+{
+  if (!qp) return;
+  memset(qp, 0, sizeof(*qp));
+  qp->empty_db = 9.5f;       // DESIGN.md 4.6: calibrated on the simulator and the recording
+  qp->single_snr_db = 8.8f;
+}
+
+int rfid_b200_window_quality(rfid_b200_ctx* ctx, const float* d_windows, const rfid_b200_window_result* d_results,
+                             const int32_t* d_counts, int nseg, int max_windows, const rfid_b200_quality_params* qp,
+                             rfid_b200_quality* d_quality, void* stream)
+{
+  if (!ctx || !d_windows || !d_results || !d_counts || !d_quality || nseg < 0 || max_windows < 0) return RFID_B200_EINVAL;
+  rfid_b200_quality_params d;
+  rfid_b200_default_quality_params(&d);
+  if (qp) d = *qp;
+  if (!std::isfinite(d.empty_db) || !std::isfinite(d.single_snr_db)) return RFID_B200_EINVAL;
+  ctx->last_launches = 0;
+  const long long slots = (long long)nseg * max_windows;
+  if (slots == 0) return RFID_B200_OK;
+  CK(cudaSetDevice(ctx->device));
+  QualityArgs A;
+  A.windows = reinterpret_cast<const float2*>(d_windows);
+  A.results = d_results; A.counts = d_counts; A.quality = d_quality;
+  A.nseg = nseg; A.max_windows = max_windows;
+  A.empty_ratio = std::pow(10.0, (double)d.empty_db / 10.0);
+  A.single_ratio = std::pow(10.0, (double)d.single_snr_db / 10.0);
+  A.cfg = ctx->cfg;
+  rx_quality_kernel<<<(unsigned)((slots + kQualityWarps - 1) / kQualityWarps), 32 * kQualityWarps, 0, (cudaStream_t)stream>>>(A);
+  CK(cudaGetLastError());
+  ctx->last_launches = 1;
   return RFID_B200_OK;
 }
 

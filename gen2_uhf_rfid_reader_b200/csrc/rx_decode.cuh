@@ -194,6 +194,28 @@ __device__ __forceinline__ float win_stream_period(const RxConfig& c, int lane)
   return f_add(c.t_min, f_div(f_mul((float)(lane < number_steps ? lane : 0), f_sub(c.t_max, c.t_min)), (float)(number_steps - 1)));
 }
 
+// The decoder's sample positions, shared with the window-quality kernel (rx_quality.cuh), which projects the same samples.
+// First data sample: sync index + 6.5 symbols (:107).
+__device__ __forceinline__ int win_data_index(const RxConfig& c, int sync_index)
+{
+  const float n = c.n_tag_bit_f;
+  return (int)f_add(f_add((float)sync_index, f_mul((float)kTagPreambleBits, n)), f_mul(n, 0.5f));
+}
+// RN16 half-bit m (:237-253): the float position index + half + ... + half (m additions, each rounded); the sample is
+// roundf of it.  win_stream_finish writes the same loop out.
+__device__ __forceinline__ float win_rn16_halfbit(int index, float half, int m)
+{
+  float jm = (float)index;
+  for (int i = 0; i < m; i++) jm = f_add(jm, half);
+  return jm;
+}
+// EPC bit j's pair (:173): a = (int)(j * (2T) + index), b = (int)(j * 2 * T + T + index)
+__device__ __forceinline__ int win_epc_pos_a(int j, float twoT, int index) { return (int)f_add(f_mul((float)j, twoT), (float)index); }
+__device__ __forceinline__ int win_epc_pos_b(int j, float T, int index)
+{
+  return (int)f_add(f_add(f_mul((float)(j * 2), T), T), (float)index);
+}
+
 __device__ __forceinline__ int win_head_samples(const RxConfig& c, int kind, int n_total, int stage_cap)
 {
   return min(stage_cap, kind == RFID_B200_RN16 ? n_total : (int)(c.sync_range + 6.0f * c.n_tag_bit_f) + 2);
@@ -271,7 +293,7 @@ __device__ __forceinline__ void win_stream_head(const RxConfig& c, int kind, con
   out.sync_index = max_index;
   out.score = max_corr;
   out.bits[0] = out.bits[1] = out.bits[2] = out.bits[3] = 0u;
-  S.index = (int)f_add(f_add((float)max_index, f_mul((float)kTagPreambleBits, n)), half);
+  S.index = win_data_index(c, max_index);
   S.head = head;
   S.h = out.h;
   S.e = 0.0f;
@@ -351,8 +373,8 @@ __device__ __forceinline__ void win_stream_decide(const RxConfig& c, const WinSr
 #pragma unroll
   for (int r = 0; r < 4; r++) {
     const int j = r * 32 + lane;
-    const int a = (int)f_add(f_mul((float)j, twoT), (float)index);
-    const int b = (int)f_add(f_add(f_mul((float)(j * 2), T), T), (float)index);
+    const int a = win_epc_pos_a(j, twoT, index);
+    const int b = win_epc_pos_b(j, T, index);
     ia[r] = a >= 0 && a < n_avail;
     ib[r] = b >= 0 && b < n_avail;
     wa[r] = ia[r] ? __ldcg(gw.at(a)) : dc;
@@ -393,7 +415,7 @@ __device__ __forceinline__ void win_stream_finish(const RxConfig& c, int kind, c
   const int index = S.index;
   const float2 h = S.h;
   if (kind == RFID_B200_RN16) {
-    float jm = (float)index;
+    float jm = (float)index;   // win_rn16_halfbit(index, half, lane), written out: called, it moves spills in rx_pack_kernel<sc16>
     for (int m = 0; m < lane; m++) jm = f_add(jm, half);
     bool have = jm < (float)n_avail;
     unsigned have_mask = __ballot_sync(0xffffffffu, have);

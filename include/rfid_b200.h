@@ -392,6 +392,70 @@ RFID_B200_API int rfid_b200_decode_commands_host(rfid_b200_ctx* ctx, const float
                                                  int max_commands_per_segment, rfid_b200_command* h_cmds,
                                                  int32_t* h_counts);
 
+/* ---------------- capture mode: reply quality and slot outcome ----------------
+ * The decoder says which bits a window holds, never whether a tag answered.  rfid_b200_window_quality measures the
+ * reply of every stored window and classifies its slot as empty, one reply or a collision.  It works per stored window
+ * on the window's DC-removed samples w[0, n), n = min(length, window_length(EPC)) -- what the window tap
+ * (rfid_b200_set_window_tap) holds and the decoder read -- and on the record's sync_index, h, T and length:
+ *   - projections r_j = c_proj(s_a, s_b, h) = Re((s_a - s_b) * conj(h)) in float with every operation rounded, the
+ *     floats whose signs the decoder turned into bits, at the decoder's own positions (a sample outside [0, n) is 0):
+ *       RN16, k = 16: s_a, s_b = w[roundf(jm_2j)], w[roundf(jm_2j+1)], jm_0 = index, jm_m+1 = jm_m + n_tag_bit/2;
+ *       EPC, k = 128: a = (int)(j*(2T) + index), b = (int)(j*2*T + T + index);
+ *     index = (int)(sync_index + 6*n_tag_bit + n_tag_bit/2).  An RN16 window with a half-bit jm_0..31 >= n (the
+ *     decoder's crc_ok = -2) gets energy = snr = NaN, n_decisions = 0 and outcome EMPTY;
+ *   - snr = m*m / (S2/k - m*m), m = S1/k, S1 = sum |r_j|, S2 = sum r_j*r_j in double (r*r of a float is exact); a zero
+ *     denominator gives +inf;
+ *   - energy = (Er / (r1 - sync_index)) / (En / m): Er = sum |w|^2 over the reply [sync_index, r1), En over the noise
+ *     reference, m its sample count, |w|^2 = re*re + im*im in double (both squares exact).  With n_i = n_tag_bit_i:
+ *     e = the decoder's position two half-bits after its last decision sample, + n_i/5 (integer division): RN16
+ *     roundf(jm_33) + n_i/5, EPC (int)(128*2*T + T + index) + n_i/5 (the last decision sample lies in the first half of
+ *     the dummy 1 a tag appends to every reply; e is past its second half and the matched filter's response to it).
+ *     The reply begins about half a bit before sync_index, so the reference is the head [0, h) with
+ *     h = min(max(sync_index - 2*n_i/5, 0), n), then the tail [t, n) with t = min(e, n); when h + n - t < n_i,
+ *     t = max(n - (n_i - h), h) (the tail moved back into the reply's end).  r1 = min(e, t).  At every sync index the
+ *     preamble search can return and every well-defined rate with decimation 5, an RN16 reference holds at least n_i
+ *     samples before or after the reply, so a late reply is measured like an early one; an EPC reply of a slow tag
+ *     clock (T near its maximum) can reach the end of its window, and then part of the reference lies in it and the
+ *     energy reads low.  A record with sync_index < 0, r1 <= sync_index or m = 0 gets energy NaN;
+ *   - every sum has one order: term i to lane i % 32 (i ascending within a lane, from 0.0), then the 32 lane sums in
+ *     ascending lane order; all arithmetic in double with round-to-nearest, snr and energy rounded once to float (one
+ *     NaN pattern, 0x7fc00000).  They are linear ratios; convert to dB for display;
+ *   - outcome: EMPTY unless energy >= empty_ratio (so also for NaN); then an RN16 window is SINGLE if snr >=
+ *     single_ratio, else COLLISION; an EPC window is SINGLE (a collision is a property of the RN16 slot).  The
+ *     thresholds are pow(10, dB / 10) in double of the float parameters, compared with the stored floats.
+ * Defaults (calibrated on the simulators and on the reference's recording, its replies also moved up to 9 samples
+ * later in their windows; DESIGN.md 4.6): empty_db 9.5 lies between the loudest empty slot of the closed-loop
+ * simulator (9.0 dB) and the recording's weakest reply (9.8 dB); single_snr_db 8.8 lies below the simulators' weakest
+ * single reply (9.0 dB) and above all but a few of their collided slots. */
+enum { RFID_B200_SLOT_EMPTY = 0, RFID_B200_SLOT_SINGLE = 1, RFID_B200_SLOT_COLLISION = 2 };
+
+typedef struct rfid_b200_quality_params {
+  float empty_db;      /* finite; 9.5 */
+  float single_snr_db; /* finite; 8.8 */
+  int32_t reserved[6];
+} rfid_b200_quality_params;
+
+/* One window's quality (16 bytes), at the index of its window record.  (Named without "window_" because that is the
+ * entry point's name.) */
+typedef struct rfid_b200_quality {
+  float energy, snr;   /* linear ratios (rule above) */
+  int32_t outcome;     /* RFID_B200_SLOT_* */
+  int32_t n_decisions; /* 16 (RN16), 128 (EPC), 0 (no RN16 decision) */
+} rfid_b200_quality;
+
+RFID_B200_API void rfid_b200_default_quality_params(rfid_b200_quality_params* qp);
+
+/* Quality records of the stored windows of a decode_capture call (device pointers, asynchronous on `stream`):
+ * d_windows = the window tap the call wrote (set before it with rfid_b200_set_window_tap, nseg * max_windows *
+ * window_length(EPC) complex samples), d_results / d_counts its records and counts.  Record k of segment s goes to
+ * d_quality[s * max_windows + k] for k < min(d_counts[s], max_windows); nothing else is written.  qp NULL = defaults.
+ * Returns RFID_B200_EINVAL for a NULL pointer, non-finite thresholds and negative counts.  One warp per record slot
+ * reads its window once. */
+RFID_B200_API int rfid_b200_window_quality(rfid_b200_ctx* ctx, const float* d_windows,
+                                           const rfid_b200_window_result* d_results, const int32_t* d_counts, int nseg,
+                                           int max_windows, const rfid_b200_quality_params* qp,
+                                           rfid_b200_quality* d_quality, void* stream);
+
 /* ---------------- block mode (GNU Radio drop-in) ----------------
  * Called from the thin host blocks' general_work(); HOST pointers, owned by the
  * scheduler, touched only during the call.  State lives in the context (device
