@@ -113,6 +113,26 @@ QUALITY_DTYPE = np.dtype([("energy", "<f4"), ("snr", "<f4"), ("outcome", "<i4"),
 assert QUALITY_DTYPE.itemsize == C.sizeof(Quality) == 16 and C.sizeof(QualityParams) == 32
 
 
+FIX_CRC_OK, FIX_RECOVERED, FIX_AMBIGUOUS, FIX_FAILED, FIX_SKIPPED, FIX_NOT_EPC = range(6)
+
+
+class RecoverParams(C.Structure):
+    """rfid_b200_recover_params (include/rfid_b200.h): P least reliable positions, at most W flips, SNR gate in dB."""
+    _fields_ = [("positions", C.c_int32), ("max_flips", C.c_int32), ("min_snr_db", C.c_float),
+                ("reserved", C.c_int32 * 5)]
+
+
+class EpcFix(C.Structure):
+    _fields_ = [("status", C.c_int32), ("n_flips", C.c_int32), ("n_pass", C.c_int32), ("cost", C.c_float),
+                ("bits", C.c_uint8 * 16)]
+
+
+#: numpy view of rfid_b200_epc_fix (32 bytes): RFID_B200_FIX_* status, flips, passing candidates, cost, bits
+EPC_FIX_DTYPE = np.dtype([("status", "<i4"), ("n_flips", "<i4"), ("n_pass", "<i4"), ("cost", "<f4"),
+                          ("bits", "u1", (16,))])
+assert EPC_FIX_DTYPE.itemsize == C.sizeof(EpcFix) == 32 and C.sizeof(RecoverParams) == 32
+
+
 def make_segments(offsets, lengths):
     segs = np.zeros(len(offsets), dtype=SEGMENT_DTYPE)
     segs["offset"] = np.asarray(offsets, dtype=np.uint64)

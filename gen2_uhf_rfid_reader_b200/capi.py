@@ -110,6 +110,9 @@ def load_library():
     L.rfid_b200_default_quality_params.argtypes = [C.POINTER(abi.QualityParams)]
     L.rfid_b200_window_quality.restype = C.c_int
     L.rfid_b200_window_quality.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.POINTER(abi.QualityParams), vp, vp]
+    L.rfid_b200_default_recover_params.argtypes = [C.POINTER(abi.RecoverParams)]
+    L.rfid_b200_recover_epc.restype = C.c_int
+    L.rfid_b200_recover_epc.argtypes = [vp, vp, vp, vp, vp, C.c_int, C.c_int, C.POINTER(abi.RecoverParams), vp, vp]
     _lib = L
     return L
 
@@ -125,6 +128,7 @@ EXPORTED_SYMBOLS = [
     "rfid_b200_decode_capture_sc16", "rfid_b200_segment_capture_sc16", "rfid_b200_ingest_capture_host_sc16",
     "rfid_b200_default_cmd_params", "rfid_b200_decode_commands", "rfid_b200_decode_commands_sc16",
     "rfid_b200_decode_commands_host", "rfid_b200_default_quality_params", "rfid_b200_window_quality",
+    "rfid_b200_default_recover_params", "rfid_b200_recover_epc",
 ]
 
 
@@ -169,6 +173,16 @@ def default_quality_params(**kw):
     for k, v in kw.items():
         setattr(qp, k, type(getattr(qp, k))(v))
     return qp
+
+
+def default_recover_params(**kw):
+    """rfid_b200_recover_params with the library's defaults (positions 12, max_flips 4, min_snr_db 7.0), fields set by
+    kw."""
+    rp = abi.RecoverParams()
+    load_library().rfid_b200_default_recover_params(C.byref(rp))
+    for k, v in kw.items():
+        setattr(rp, k, type(getattr(rp, k))(v))
+    return rp
 
 
 def default_params(**kw):
@@ -326,16 +340,50 @@ class Gen2Rx:
         device memory (3.5 GB for 160,000 segments of 2 windows at 2 MS/s); it is released to torch's stream-ordered
         allocator on return, so the call stays asynchronous on the current stream like `decode_capture`.  Returns
         (results, counts, quality) as device tensors."""
+        tap, results, counts = self._decode_tapped(iq, segs, max_windows, scale)
+        return results, counts, self.window_quality(tap, results, counts, max_windows, params=params)
+
+    def _decode_tapped(self, iq, segs, max_windows, scale):
+        """`decode_capture` with a window tap set for this one call: (tap, results, counts)"""
         import torch
         nseg = segs.numel() * segs.element_size() // 16
         tap = torch.empty(nseg * max_windows * self.len_epc, dtype=torch.complex64, device=iq.device)
         self.set_window_tap(tap)
         try:
             results, counts = self.decode_capture(iq, segs, max_windows=max_windows, scale=scale)
-            quality = self.window_quality(tap, results, counts, max_windows, params=params)
         finally:
             self.set_window_tap(None)
-        return results, counts, quality
+        return tap, results, counts
+
+    # ---------------------------------------------------------------- capture mode: EPC replies that fail their CRC
+    def recover_epc(self, windows, results, counts, quality, max_windows, params=None, fixes=None, stream=None):
+        """Recovery records (rule: include/rfid_b200.h) of the stored windows of a `decode_capture` call: windows, results
+        and counts as in `window_quality`, quality its output for them; params: `RecoverParams` (None: defaults, see
+        `default_recover_params`).  Asynchronous on `stream`.  Returns fixes, a CUDA uint8 tensor [nseg * max_windows,
+        32] (`fixes_to_numpy` views it as EPC_FIX_DTYPE); slots beyond a segment's stored records are left as they were
+        (zero when allocated here).  `apply_fixes` folds the RECOVERED windows into the records."""
+        import torch
+        nseg = counts.numel()
+        if windows.numel() * windows.element_size() < nseg * max_windows * self.len_epc * 8:
+            raise ValueError("the window tap holds fewer than nseg * max_windows * len_epc complex samples")
+        if fixes is None:
+            fixes = torch.zeros((nseg * max_windows, 32), dtype=torch.uint8, device=results.device)
+        s = stream if stream is not None else torch.cuda.current_stream(results.device)
+        rp = C.byref(params) if params is not None else None
+        rc = self.lib.rfid_b200_recover_epc(self.h, windows.data_ptr(), results.data_ptr(), counts.data_ptr(),
+                                            quality.data_ptr(), nseg, max_windows, rp, fixes.data_ptr(), s.cuda_stream)
+        self._ck(rc, "rfid_b200_recover_epc")
+        return fixes
+
+    def decode_capture_recover(self, iq, segs, max_windows=2, quality_params=None, recover_params=None,
+                               scale=SC16_SCALE):
+        """`decode_capture` with the window tap set for this one call, then `window_quality` and `recover_epc` on what it
+        wrote; iq, segs and scale as in `decode_capture` (fc32 or sc16), the tap as in `decode_capture_quality`.
+        Returns (results, counts, quality, fixes) as device tensors; the records are the decoder's, unchanged."""
+        tap, results, counts = self._decode_tapped(iq, segs, max_windows, scale)
+        quality = self.window_quality(tap, results, counts, max_windows, params=quality_params)
+        fixes = self.recover_epc(tap, results, counts, quality, max_windows, params=recover_params)
+        return results, counts, quality, fixes
 
     # ---------------------------------------------------------------- capture ingest
     def segment_capture(self, iq, segmenter=None, capacity=None, stream=None, scale=SC16_SCALE):
@@ -552,6 +600,29 @@ def quality_to_numpy(quality, counts, max_windows):
     q = quality.cpu().numpy().reshape(-1).view(abi.QUALITY_DTYPE)
     c = counts.cpu().numpy()
     return q.reshape(c.size, max_windows), c
+
+
+def fixes_to_numpy(fixes, counts, max_windows):
+    """device uint8[nseg*max_windows,32] + int32[nseg] -> (EPC_FIX_DTYPE[nseg,max_windows], int32[nseg])"""
+    f = fixes.cpu().numpy().reshape(-1).view(abi.EPC_FIX_DTYPE)
+    c = counts.cpu().numpy()
+    return f.reshape(c.size, max_windows), c
+
+
+def apply_fixes(recs, counts, fixes):
+    """A copy of the records (RESULT_DTYPE[nseg, max_windows], host numpy) in which every stored RECOVERED window
+    (`recover_epc` output, EPC_FIX_DTYPE[nseg, max_windows]) has the corrected bits, crc_ok = 1 and tag_id = bits
+    104..111, as the decoder sets them for a passing EPC; `reduce_stats`, `transcript` and `slot_table` then count
+    recovered reads like any other."""
+    out = np.array(recs, dtype=abi.RESULT_DTYPE, copy=True)
+    fixes = np.asarray(fixes, dtype=abi.EPC_FIX_DTYPE)
+    counts = np.asarray(counts)
+    stored = np.arange(out.shape[1])[None, :] < np.minimum(np.maximum(counts, 0), out.shape[1])[:, None]
+    fix = stored & (fixes["status"] == abi.FIX_RECOVERED)
+    out["bits"][fix] = fixes["bits"][fix]
+    out["crc_ok"][fix] = 1
+    out["tag_id"][fix] = fixes["bits"][fix][:, 13]
+    return out
 
 
 #: one row per segment: what its RN16 and EPC windows say about the slot (see `slot_table`)

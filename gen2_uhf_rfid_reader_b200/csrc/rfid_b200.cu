@@ -20,6 +20,7 @@
 #include "rx_ingest.cuh"
 #include "rx_pack.cuh"
 #include "rx_quality.cuh"
+#include "rx_recover.cuh"
 #include "tx_synth.cuh"
 
 using namespace rfid_b200;
@@ -1381,6 +1382,51 @@ int rfid_b200_window_quality(rfid_b200_ctx* ctx, const float* d_windows, const r
   A.single_ratio = std::pow(10.0, (double)d.single_snr_db / 10.0);
   A.cfg = ctx->cfg;
   rx_quality_kernel<<<(unsigned)((slots + kQualityWarps - 1) / kQualityWarps), 32 * kQualityWarps, 0, (cudaStream_t)stream>>>(A);
+  CK(cudaGetLastError());
+  ctx->last_launches = 1;
+  return RFID_B200_OK;
+}
+
+// ------------------------------------------------------------------ capture mode: EPC replies that fail their CRC
+void rfid_b200_default_recover_params(rfid_b200_recover_params* rp)
+{
+  if (!rp) return;
+  memset(rp, 0, sizeof(*rp));
+  rp->positions = 12;
+  rp->max_flips = 4;
+  rp->min_snr_db = 7.0f;   // DESIGN.md 4.7: above the EPC windows of empty slots and the replies that recover wrongly
+}
+
+int rfid_b200_recover_epc(rfid_b200_ctx* ctx, const float* d_windows, const rfid_b200_window_result* d_results,
+                          const int32_t* d_counts, const rfid_b200_quality* d_quality, int nseg, int max_windows,
+                          const rfid_b200_recover_params* rp, rfid_b200_epc_fix* d_fix, void* stream)
+{
+  if (!ctx || !d_windows || !d_results || !d_counts || !d_quality || !d_fix || nseg < 0 || max_windows < 0)
+    return RFID_B200_EINVAL;
+  rfid_b200_recover_params d;
+  rfid_b200_default_recover_params(&d);
+  if (rp) d = *rp;
+  if (d.positions < 1 || d.positions > kRecoverMaxPositions || d.max_flips < 1 || d.max_flips > d.positions ||
+      !std::isfinite(d.min_snr_db))
+    return RFID_B200_EINVAL;
+  long long n_candidates = 0, binom = 1;
+  for (int k = 1; k <= d.max_flips; k++) {   // binomial(P, k), exact: binomial(P, k - 1) * (P - k + 1) is divisible by k
+    binom = binom * (d.positions - k + 1) / k;
+    n_candidates += binom;
+  }
+  if (n_candidates > kRecoverMaxCandidates) return RFID_B200_EINVAL;
+  ctx->last_launches = 0;
+  const long long slots = (long long)nseg * max_windows;
+  if (slots == 0) return RFID_B200_OK;
+  CK(cudaSetDevice(ctx->device));
+  RecoverArgs A;
+  A.windows = reinterpret_cast<const float2*>(d_windows);
+  A.results = d_results; A.counts = d_counts; A.quality = d_quality; A.fix = d_fix;
+  A.nseg = nseg; A.max_windows = max_windows;
+  A.positions = d.positions; A.max_flips = d.max_flips; A.n_candidates = (int)n_candidates;
+  A.min_snr_ratio = std::pow(10.0, (double)d.min_snr_db / 10.0);
+  A.cfg = ctx->cfg;
+  rx_recover_kernel<<<(unsigned)((slots + kRecoverWarps - 1) / kRecoverWarps), 32 * kRecoverWarps, 0, (cudaStream_t)stream>>>(A);
   CK(cudaGetLastError());
   ctx->last_launches = 1;
   return RFID_B200_OK;

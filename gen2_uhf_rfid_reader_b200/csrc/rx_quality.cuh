@@ -43,6 +43,17 @@ __device__ __forceinline__ double quality_power_sum(const float2* w, int h1, int
   return quality_lane_sum(part);
 }
 
+// EPC decision j's projection r_j = c_proj(s_a, s_b, h) at the decoder's positions, a sample outside [0, n) taken as 0
+// (the window-quality and EPC-recovery rules both use it)
+__device__ __forceinline__ float epc_projection(const float2* w, int n, int j, float T, float twoT, int index, float2 h)
+{
+  const float2 zero = make_float2(0.0f, 0.0f);
+  const int pa = win_epc_pos_a(j, twoT, index), pb = win_epc_pos_b(j, T, index);
+  const float2 sa = (pa >= 0 && pa < n) ? __ldg(w + pa) : zero;
+  const float2 sb = (pb >= 0 && pb < n) ? __ldg(w + pb) : zero;
+  return c_proj(sa, sb, h);
+}
+
 __device__ __forceinline__ float quality_canonical(double v)
 {
   return v != v ? __int_as_float(0x7fc00000) : __double2float_rn(v);   // (one NaN pattern, numpy's)
@@ -91,11 +102,7 @@ __global__ void __launch_bounds__(32 * kQualityWarps) rx_quality_kernel(const Qu
     const float T = rec.T, twoT = f_mul(2.0f, T);
 #pragma unroll
     for (int q = 0; q < 4; q++) {
-      const int j = q * 32 + lane;
-      const int pa = win_epc_pos_a(j, twoT, index), pb = win_epc_pos_b(j, T, index);
-      const float2 sa = (pa >= 0 && pa < n) ? __ldg(w + pa) : zero;
-      const float2 sb = (pb >= 0 && pb < n) ? __ldg(w + pb) : zero;
-      const double d = c_proj(sa, sb, h);
+      const double d = epc_projection(w, n, q * 32 + lane, T, twoT, index, h);
       a1 = __dadd_rn(a1, fabs(d));
       a2 = __dadd_rn(a2, __dmul_rn(d, d));
     }

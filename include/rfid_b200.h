@@ -456,6 +456,76 @@ RFID_B200_API int rfid_b200_window_quality(rfid_b200_ctx* ctx, const float* d_wi
                                            int max_windows, const rfid_b200_quality_params* qp,
                                            rfid_b200_quality* d_quality, void* stream);
 
+/* ---------------- capture mode: EPC replies that fail their CRC ----------------
+ * One wrong sign among an EPC window's 128 decisions loses the read.  rfid_b200_recover_epc flips the least reliable
+ * decisions of a failing EPC window and keeps the result when exactly one flip set makes the window pass.  Per stored
+ * window slot (s, k), k < min(count, max_windows), of a decode_capture call, from that call's window tap, records and
+ * rfid_b200_window_quality records:
+ *   1. an RN16 window: status NOT_EPC, the record's bits;
+ *   2. an EPC window with crc_ok == 1: status CRC_OK, the record's bits (the tap is not read);
+ *   3. a failing EPC window is SKIPPED unless its quality record has n_decisions == 128 and snr >= min_snr_ratio
+ *      (NaN: SKIPPED), min_snr_ratio = pow(10, min_snr_db / 10) in double of the float parameter, compared with the
+ *      stored float (the convention of the quality thresholds);
+ *   4. otherwise a recovery is attempted:
+ *      - the projections r_j, j = 0..127, exactly as the quality rule computes them (c_proj at win_epc_pos_a/b, a
+ *        sample outside [0, n) taken as 0).  Their signs s_j = r_j > 0 are the record's bits through
+ *        bit_j = s_j xor s_(j-1), s_(-1) = 1;
+ *      - reliability p_j = |r_j| (float); the P = `positions` least reliable positions, ordered by (p_j, j) ascending;
+ *      - candidates: every subset F of those P positions with 1 <= |F| <= W = `max_flips`.  Flipping s_j flips bits j
+ *        and j + 1 (for j = 127 bit 127 only);
+ *      - a candidate passes iff its bits pass the decoder's CRC-16 (bytes 0..13 against bytes 14..15) and its PC bits
+ *        0..4 (the EPC length field, MSB first) are 00110: 6 words, the 96-bit EPC a 128-bit window holds;
+ *      - n_pass = the number of passing candidates.  RECOVERED iff n_pass == 1: the record gets the corrected bits,
+ *        n_flips = |F| and cost = (sum of p_j over F in double, ascending j) / (S1 / 128), rounded once to float, with
+ *        S1 = sum of |r_j| in double in the quality rule's order.  AMBIGUOUS iff n_pass >= 2, FAILED iff n_pass == 0.
+ * Every status but RECOVERED stores the record's bits, n_flips = 0 and cost = NaN (0x7fc00000); n_pass is 0 unless a
+ * recovery was attempted.  The result does not depend on the order the candidates are tried in.
+ * False accepts: a window whose true error set is not a candidate passes each candidate with probability about 2^-21
+ * (16 CRC bits and 5 length bits) when its bits are random, so it is RECOVERED wrongly with probability at most
+ * C * 2^-21, C = sum over k = 1..W of binomial(P, k); at the defaults P = 12, W = 4, C = 793: 3.8e-4.  A real reply's
+ * length field is usually decoded right, and a candidate that flips no sign in 0..4 leaves it right, so for such a
+ * window only the 16 CRC bits test the candidate: at most C * 2^-16, 1.2 % at the defaults.  The SNR gate keeps the
+ * attempts to windows whose few errors are likely candidates.
+ * Default min_snr_db 7.0 (DESIGN.md 4.7): the EPC windows of empty slots reach about 4.2 dB (pure noise: about
+ * 2.4 dB); below 7 dB the simulated weak tag's failing replies gave wrong unique passes, above it none. */
+enum {
+  RFID_B200_FIX_CRC_OK = 0,
+  RFID_B200_FIX_RECOVERED = 1,
+  RFID_B200_FIX_AMBIGUOUS = 2,
+  RFID_B200_FIX_FAILED = 3,
+  RFID_B200_FIX_SKIPPED = 4,
+  RFID_B200_FIX_NOT_EPC = 5
+};
+
+typedef struct rfid_b200_recover_params {
+  int32_t positions;   /* P: 1..32; 12 */
+  int32_t max_flips;   /* W: 1..P; 4 */
+  float min_snr_db;    /* finite; 7.0 */
+  int32_t reserved[5];
+} rfid_b200_recover_params;
+
+/* One window's recovery (32 bytes), at the index of its window record. */
+typedef struct rfid_b200_epc_fix {
+  int32_t status;   /* RFID_B200_FIX_* */
+  int32_t n_flips;  /* |F| of a RECOVERED window, else 0 */
+  int32_t n_pass;   /* passing candidates of an attempted window, else 0 */
+  float cost;       /* RECOVERED: flipped reliability over the mean reliability; else NaN */
+  uint8_t bits[16]; /* corrected (RECOVERED) or the record's bits */
+} rfid_b200_epc_fix;
+
+RFID_B200_API void rfid_b200_default_recover_params(rfid_b200_recover_params* rp);
+
+/* Recovery records of the stored windows of a decode_capture call (device pointers, asynchronous on `stream`):
+ * d_windows / d_results / d_counts as for rfid_b200_window_quality, d_quality its output for the same windows.  Record k
+ * of segment s goes to d_fix[s * max_windows + k] for k < min(d_counts[s], max_windows); nothing else is written.
+ * rp NULL = defaults.  Returns RFID_B200_EINVAL for a NULL pointer, negative counts, P outside 1..32, W outside 1..P,
+ * a non-finite min_snr_db, or more than 65536 candidates.  One warp per record slot; only attempted windows read the
+ * tap. */
+RFID_B200_API int rfid_b200_recover_epc(rfid_b200_ctx* ctx, const float* d_windows,
+                                        const rfid_b200_window_result* d_results, const int32_t* d_counts,
+                                        const rfid_b200_quality* d_quality, int nseg, int max_windows,
+                                        const rfid_b200_recover_params* rp, rfid_b200_epc_fix* d_fix, void* stream);
+
 /* ---------------- block mode (GNU Radio drop-in) ----------------
  * Called from the thin host blocks' general_work(); HOST pointers, owned by the
  * scheduler, touched only during the call.  State lives in the context (device
