@@ -133,6 +133,34 @@ EPC_FIX_DTYPE = np.dtype([("status", "<i4"), ("n_flips", "<i4"), ("n_pass", "<i4
 assert EPC_FIX_DTYPE.itemsize == C.sizeof(EpcFix) == 32 and C.sizeof(RecoverParams) == 32
 
 
+class ReportParams(C.Structure):
+    """rfid_b200_report_params (include/rfid_b200.h): reject reads whose PC length field is not 6 words."""
+    _fields_ = [("check_length", C.c_int32), ("reserved", C.c_int32 * 7)]
+
+
+class Tag(C.Structure):
+    _fields_ = [("epc", C.c_uint8 * 16), ("reads", C.c_int32), ("recovered", C.c_int32), ("first_slot", C.c_int32),
+                ("last_slot", C.c_int32), ("peak_slot", C.c_int32), ("peak_power", C.c_float),
+                ("last_h_re", C.c_float), ("last_h_im", C.c_float), ("first_time", C.c_int64),
+                ("last_time", C.c_int64)]
+
+
+class TagSummary(C.Structure):
+    _fields_ = [("n_tags", C.c_int32), ("reads", C.c_int32), ("recovered", C.c_int32), ("rejected_length", C.c_int32),
+                ("rejected_empty", C.c_int32), ("reserved", C.c_int32 * 3)]
+
+
+#: numpy view of rfid_b200_tag (64 bytes): one tag of the inventory report
+TAG_DTYPE = np.dtype([("epc", "u1", (16,)), ("reads", "<i4"), ("recovered", "<i4"), ("first_slot", "<i4"),
+                      ("last_slot", "<i4"), ("peak_slot", "<i4"), ("peak_power", "<f4"), ("last_h_re", "<f4"),
+                      ("last_h_im", "<f4"), ("first_time", "<i8"), ("last_time", "<i8")])
+#: numpy view of rfid_b200_tag_summary (32 bytes)
+TAG_SUMMARY_DTYPE = np.dtype([("n_tags", "<i4"), ("reads", "<i4"), ("recovered", "<i4"), ("rejected_length", "<i4"),
+                              ("rejected_empty", "<i4"), ("reserved", "<i4", (3,))])
+assert TAG_DTYPE.itemsize == C.sizeof(Tag) == 64 and TAG_SUMMARY_DTYPE.itemsize == C.sizeof(TagSummary) == 32
+assert C.sizeof(ReportParams) == 32
+
+
 def make_segments(offsets, lengths):
     segs = np.zeros(len(offsets), dtype=SEGMENT_DTYPE)
     segs["offset"] = np.asarray(offsets, dtype=np.uint64)

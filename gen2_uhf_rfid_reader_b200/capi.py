@@ -113,6 +113,10 @@ def load_library():
     L.rfid_b200_default_recover_params.argtypes = [C.POINTER(abi.RecoverParams)]
     L.rfid_b200_recover_epc.restype = C.c_int
     L.rfid_b200_recover_epc.argtypes = [vp, vp, vp, vp, vp, C.c_int, C.c_int, C.POINTER(abi.RecoverParams), vp, vp]
+    L.rfid_b200_default_report_params.argtypes = [C.POINTER(abi.ReportParams)]
+    L.rfid_b200_tag_report.restype = C.c_int
+    L.rfid_b200_tag_report.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, vp, vp, C.POINTER(abi.ReportParams), C.c_int,
+                                       vp, vp, vp, vp]
     _lib = L
     return L
 
@@ -128,7 +132,8 @@ EXPORTED_SYMBOLS = [
     "rfid_b200_decode_capture_sc16", "rfid_b200_segment_capture_sc16", "rfid_b200_ingest_capture_host_sc16",
     "rfid_b200_default_cmd_params", "rfid_b200_decode_commands", "rfid_b200_decode_commands_sc16",
     "rfid_b200_decode_commands_host", "rfid_b200_default_quality_params", "rfid_b200_window_quality",
-    "rfid_b200_default_recover_params", "rfid_b200_recover_epc",
+    "rfid_b200_default_recover_params", "rfid_b200_recover_epc", "rfid_b200_default_report_params",
+    "rfid_b200_tag_report",
 ]
 
 
@@ -180,6 +185,15 @@ def default_recover_params(**kw):
     kw."""
     rp = abi.RecoverParams()
     load_library().rfid_b200_default_recover_params(C.byref(rp))
+    for k, v in kw.items():
+        setattr(rp, k, type(getattr(rp, k))(v))
+    return rp
+
+
+def default_report_params(**kw):
+    """rfid_b200_report_params with the library's defaults (check_length 1), fields set by kw."""
+    rp = abi.ReportParams()
+    load_library().rfid_b200_default_report_params(C.byref(rp))
     for k, v in kw.items():
         setattr(rp, k, type(getattr(rp, k))(v))
     return rp
@@ -384,6 +398,55 @@ class Gen2Rx:
         quality = self.window_quality(tap, results, counts, max_windows, params=quality_params)
         fixes = self.recover_epc(tap, results, counts, quality, max_windows, params=recover_params)
         return results, counts, quality, fixes
+
+    # ---------------------------------------------------------------- capture mode: the tag inventory report
+    def tag_report(self, results, counts, segs, max_windows, quality=None, fixes=None, params=None, max_tags=1024,
+                   tags=None, summary=None, read_tag=None, stream=None):
+        """The inventory report (rule: include/rfid_b200.h) of the stored slots of a `decode_capture` call: results,
+        counts its outputs, segs the segment table it decoded (CUDA tensor, see `segments_to_device`); quality its
+        `window_quality` records (None: no empty-slot rejection), fixes its `recover_epc` records (None: no recovered
+        reads); params: `ReportParams` (None: defaults, see `default_report_params`).  Asynchronous on `stream`.  Returns
+        (tags uint8[max_tags, 64], summary uint8[32], read_tag int32[nseg * max_windows]) as CUDA tensors, allocated here
+        unless given (`tags_to_numpy` views the first two); read_tag entries of slots that are not stored are left as
+        they were (-1 when allocated here)."""
+        import torch
+        nseg = counts.numel()
+        if segs.numel() * segs.element_size() < nseg * 16:
+            raise ValueError("the segment table holds fewer than nseg entries")
+        dev = results.device
+        if tags is None:
+            tags = torch.zeros((max_tags, 64), dtype=torch.uint8, device=dev)
+        if tags.numel() < max_tags * 64:
+            raise ValueError("the tag buffer holds fewer than max_tags records")
+        if summary is None:
+            summary = torch.zeros(32, dtype=torch.uint8, device=dev)
+        if read_tag is None:
+            read_tag = torch.full((nseg * max_windows,), -1, dtype=torch.int32, device=dev)
+        s = stream if stream is not None else torch.cuda.current_stream(dev)
+        rp = C.byref(params) if params is not None else None
+        rc = self.lib.rfid_b200_tag_report(self.h, segs.data_ptr(), results.data_ptr(), counts.data_ptr(), nseg,
+                                           max_windows, quality.data_ptr() if quality is not None else None,
+                                           fixes.data_ptr() if fixes is not None else None, rp, max_tags,
+                                           tags.data_ptr() if max_tags > 0 else None, summary.data_ptr(),
+                                           read_tag.data_ptr(), s.cuda_stream)
+        self._ck(rc, "rfid_b200_tag_report")
+        return tags, summary, read_tag
+
+    def decode_capture_report(self, iq, segs, max_windows=2, recover=True, reject_empty=True, quality_params=None,
+                              recover_params=None, report_params=None, max_tags=1024, scale=SC16_SCALE):
+        """`decode_capture` with the window tap set for this one call, then `window_quality`, `recover_epc` (recover=True)
+        and `tag_report` on what they wrote; iq, segs and scale as in `decode_capture` (fc32 or sc16), the tap as in
+        `decode_capture_quality`.  reject_empty: the report rejects reads in slots the quality rule calls EMPTY (CRC
+        passes on noise; but also replies weaker than quality_params.empty_db, DESIGN 4.8).  Only the report has to
+        come back to the host.  Returns (results, counts, quality, fixes, tags, summary, read_tag) as device tensors
+        (fixes None without recovery)."""
+        tap, results, counts = self._decode_tapped(iq, segs, max_windows, scale)
+        quality = self.window_quality(tap, results, counts, max_windows, params=quality_params)
+        fixes = self.recover_epc(tap, results, counts, quality, max_windows, params=recover_params) if recover else None
+        tags, summary, read_tag = self.tag_report(results, counts, segs, max_windows,
+                                                  quality=quality if reject_empty else None, fixes=fixes,
+                                                  params=report_params, max_tags=max_tags)
+        return results, counts, quality, fixes, tags, summary, read_tag
 
     # ---------------------------------------------------------------- capture ingest
     def segment_capture(self, iq, segmenter=None, capacity=None, stream=None, scale=SC16_SCALE):
@@ -622,6 +685,36 @@ def apply_fixes(recs, counts, fixes):
     out["bits"][fix] = fixes["bits"][fix]
     out["crc_ok"][fix] = 1
     out["tag_id"][fix] = fixes["bits"][fix][:, 13]
+    return out
+
+
+def tags_to_numpy(tags, summary):
+    """`tag_report` output -> (TAG_DTYPE[min(n_tags, max_tags)], TAG_SUMMARY_DTYPE record)"""
+    sm = summary.cpu().numpy().reshape(-1).view(abi.TAG_SUMMARY_DTYPE)[0]
+    t = tags.cpu().numpy().reshape(-1).view(abi.TAG_DTYPE)
+    return t[:min(int(sm["n_tags"]), t.size)].copy(), sm
+
+
+#: one row per tag of a report, in display units (see `tag_table`)
+TAG_TABLE_DTYPE = np.dtype([("epc", "U32"), ("reads", "<i4"), ("recovered", "<i4"), ("first_us", "<f8"),
+                            ("last_us", "<f8"), ("peak_rssi_db", "<f8"), ("last_phase_deg", "<f8")])
+
+
+def tag_table(tags, ntaps=25, adc_rate=2_000_000):
+    """The report's tags (TAG_DTYPE rows) in display units (host numpy only): PC + EPC + CRC as hex, reads, recovered,
+    first and last seen in microseconds from the capture's first sample (the times are raw samples at adc_rate),
+    peak_rssi_db = 10 log10(peak_power / ntaps^2), the strongest reply's power in dB relative to a full-scale sample (h
+    is a sum over the matched filter's ntaps samples), and last_phase_deg = arg(last h) in degrees."""
+    tags = np.asarray(tags, dtype=abi.TAG_DTYPE)
+    out = np.zeros(tags.size, dtype=TAG_TABLE_DTYPE)
+    out["epc"] = [bytes(bytearray(e)).hex() for e in tags["epc"]]
+    out["reads"], out["recovered"] = tags["reads"], tags["recovered"]
+    out["first_us"] = tags["first_time"] * 1e6 / adc_rate
+    out["last_us"] = tags["last_time"] * 1e6 / adc_rate
+    with np.errstate(divide="ignore", invalid="ignore"):
+        out["peak_rssi_db"] = 10.0 * np.log10(tags["peak_power"].astype(np.float64) / float(ntaps) ** 2)
+    out["last_phase_deg"] = np.degrees(np.arctan2(tags["last_h_im"].astype(np.float64),
+                                                  tags["last_h_re"].astype(np.float64)))
     return out
 
 

@@ -21,6 +21,7 @@
 #include "rx_pack.cuh"
 #include "rx_quality.cuh"
 #include "rx_recover.cuh"
+#include "rx_report.cuh"
 #include "tx_synth.cuh"
 
 using namespace rfid_b200;
@@ -81,6 +82,8 @@ struct rfid_b200_ctx {
   void* d_sim_cnt; size_t d_sim_cnt_bytes;
   // host-mode command records
   void* d_cmd; size_t d_cmd_bytes;
+  // tag report scratch: aggregates, hash table, per-slot owners, block counts
+  void* d_report; size_t d_report_bytes;
 };
 
 namespace {
@@ -412,6 +415,7 @@ int rfid_b200_create(const rfid_b200_params* p, rfid_b200_ctx** out)
   ctx->d_script = ctx->d_sim_res = ctx->d_sim_cnt = nullptr;
   ctx->d_script_bytes = ctx->d_sim_res_bytes = ctx->d_sim_cnt_bytes = 0;
   ctx->d_cmd = nullptr; ctx->d_cmd_bytes = 0;
+  ctx->d_report = nullptr; ctx->d_report_bytes = 0;
   ctx->h_stage[0] = ctx->h_stage[1] = nullptr; ctx->ev_stage[0] = ctx->ev_stage[1] = nullptr;
   memset(&ctx->layout, 0, sizeof(ctx->layout));
   memset(&ctx->layout_sc16, 0, sizeof(ctx->layout_sc16));
@@ -500,7 +504,7 @@ void rfid_b200_destroy(rfid_b200_ctx* ctx)
   if (ctx->h_blk) cudaFreeHost(ctx->h_blk);
   void* ptrs[] = {ctx->d_blk, ctx->d_win, ctx->d_yhist, ctx->d_iq, ctx->d_segs, ctx->d_res, ctx->d_cnt, ctx->d_in, ctx->d_out, ctx->d_m2, ctx->d_mf,
                   ctx->d_gate, ctx->d_gate_out, ctx->d_one, ctx->d_mask, ctx->d_chunk, ctx->d_bursts, ctx->d_ing,
-                  ctx->d_script, ctx->d_sim_res, ctx->d_sim_cnt, ctx->d_cmd};
+                  ctx->d_script, ctx->d_sim_res, ctx->d_sim_cnt, ctx->d_cmd, ctx->d_report};
   for (void* p : ptrs)
     if (p) cudaFree(p);
   for (int b = 0; b < 2; b++) {
@@ -1429,6 +1433,67 @@ int rfid_b200_recover_epc(rfid_b200_ctx* ctx, const float* d_windows, const rfid
   rx_recover_kernel<<<(unsigned)((slots + kRecoverWarps - 1) / kRecoverWarps), 32 * kRecoverWarps, 0, (cudaStream_t)stream>>>(A);
   CK(cudaGetLastError());
   ctx->last_launches = 1;
+  return RFID_B200_OK;
+}
+
+// ------------------------------------------------------------------ capture mode: the tag inventory report
+void rfid_b200_default_report_params(rfid_b200_report_params* rp)
+{
+  if (!rp) return;
+  memset(rp, 0, sizeof(*rp));
+  rp->check_length = 1;
+}
+
+int rfid_b200_tag_report(rfid_b200_ctx* ctx, const rfid_b200_segment* d_segs, const rfid_b200_window_result* d_results,
+                         const int32_t* d_counts, int nseg, int max_windows, const rfid_b200_quality* d_quality,
+                         const rfid_b200_epc_fix* d_fix, const rfid_b200_report_params* rp, int max_tags,
+                         rfid_b200_tag* d_tags, rfid_b200_tag_summary* d_summary, int32_t* d_read_tag, void* stream)
+{
+  if (!ctx || !d_segs || !d_results || !d_counts || !d_summary || (!d_tags && max_tags > 0) || nseg < 0 ||
+      max_windows < 0 || max_tags < 0)
+    return RFID_B200_EINVAL;
+  const long long slots = (long long)nseg * max_windows;
+  if (slots >= (1ll << 31)) return RFID_B200_EINVAL;
+  rfid_b200_report_params d;
+  rfid_b200_default_report_params(&d);
+  if (rp) d = *rp;
+  if (d.check_length != 0 && d.check_length != 1) return RFID_B200_EINVAL;
+  ctx->last_launches = 0;
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  CK(cudaMemsetAsync(d_summary, 0, sizeof(rfid_b200_tag_summary), st));
+  if (slots == 0) return RFID_B200_OK;
+  // scratch: aggregates [slots] | hash table [pow2 >= 2 slots] | rep [slots] | block counts; the first two start zeroed
+  const int n_blocks = (int)((slots + kReportBlockSlots - 1) / kReportBlockSlots);
+  unsigned long long buckets = 64;
+  while (buckets < 2ull * (unsigned long long)slots) buckets <<= 1;
+  const size_t agg_bytes = (size_t)slots * sizeof(ReportAgg), table_bytes = (size_t)buckets * 4;
+  const size_t rep_bytes = (size_t)slots * 4, need = agg_bytes + table_bytes + rep_bytes + (size_t)n_blocks * 4;
+  int rc;
+  if ((rc = grow(ctx, &ctx->d_report, &ctx->d_report_bytes, need))) return rc;
+  char* base = static_cast<char*>(ctx->d_report);
+  CK(cudaMemsetAsync(base, 0, agg_bytes + table_bytes, st));
+  ReportArgs A;
+  A.segs = d_segs; A.results = d_results; A.counts = d_counts; A.quality = d_quality; A.fix = d_fix;
+  A.tags = d_tags; A.summary = d_summary; A.read_tag = d_read_tag;
+  A.agg = reinterpret_cast<ReportAgg*>(base);
+  A.table = reinterpret_cast<unsigned*>(base + agg_bytes);
+  A.rep = reinterpret_cast<int32_t*>(base + agg_bytes + table_bytes);
+  A.block_count = reinterpret_cast<int32_t*>(base + agg_bytes + table_bytes + rep_bytes);
+  A.max_windows = max_windows; A.n_slots = (int)slots; A.n_blocks = n_blocks; A.max_tags = max_tags;
+  A.check_length = d.check_length; A.decim = ctx->params.decim;
+  A.table_mask = (unsigned)(buckets - 1);
+  rx_report_insert_kernel<<<n_blocks, 32 * kReportWarps, 0, st>>>(A);
+  rx_report_count_kernel<<<n_blocks, kReportThreads, 0, st>>>(A);
+  rx_report_scan_kernel<<<1, kReportScanThreads, 0, st>>>(A);
+  rx_report_write_kernel<<<n_blocks, kReportThreads, 0, st>>>(A, false);
+  int launches = 4;
+  if (d_read_tag) {
+    rx_report_write_kernel<<<n_blocks, kReportThreads, 0, st>>>(A, true);
+    launches++;
+  }
+  CK(cudaGetLastError());
+  ctx->last_launches = launches;
   return RFID_B200_OK;
 }
 

@@ -526,6 +526,71 @@ RFID_B200_API int rfid_b200_recover_epc(rfid_b200_ctx* ctx, const float* d_windo
                                         const rfid_b200_quality* d_quality, int nseg, int max_windows,
                                         const rfid_b200_recover_params* rp, rfid_b200_epc_fix* d_fix, void* stream);
 
+/* ---------------- capture mode: the tag inventory report ----------------
+ * Which tags were read, how often, when and how strongly: one entry per full PC + EPC (the records' READER_STATS,
+ * rfid_b200_reduce_stats, keys a tag by the 8 bits 104..111 as the reference does).  Built on the device from the records
+ * and counts of a decode_capture call and, optionally, its quality and recovery records.  Only stored slots are read:
+ * slot i = s * max_windows + k with k < min(max(count[s], 0), max_windows).
+ *   - candidate: an EPC record with crc_ok == 1 (key = the record's bits), or else, with d_fix given, a slot whose fix has
+ *     status RFID_B200_FIX_RECOVERED (key = the fix's bits; such a read is `recovered`);
+ *   - a candidate is rejected for its length when check_length is 1 and PC bits 0..4 are not 00110 ((key[0] >> 3) != 6:
+ *     a 128-bit window holds exactly the 6-word EPC), else for an empty slot when d_quality is given and the slot's outcome
+ *     is RFID_B200_SLOT_EMPTY.  Every other candidate is a read;
+ *   - the key is all 16 bytes (PC + EPC + CRC-16).  Tags are numbered 0, 1, ... in the order of their first read by
+ *     ascending slot index (with a table in capture order: first seen first), whatever the launch geometry;
+ *   - per tag: reads, recovered; first_slot, last_slot = smallest and largest slot of its reads; peak_slot = the read with
+ *     the largest p = (float)((double)h_re*h_re + (double)h_im*h_im) (both squares exact, the sum rounded in double, then
+ *     to float), the lowest slot on ties, a NaN p below every number; peak_power = its p (0x7fc00000 when every p of the
+ *     tag is NaN); last_h = h of the last read, whose argument is the tag's latest carrier phase; first_time, last_time =
+ *     the raw-sample time of the first and last read: segs[s].offset + decim * (open_index + sync_index) in int64 (two's
+ *     complement wrap-around), s the slot's table position (the record's segment field is not read): where the reply
+ *     starts, in samples of the capture the table indexes.  Every field is an order-independent aggregate, so the report
+ *     does not depend on the order the device runs in;
+ *   - summary: n_tags counts every tag, also those at index >= max_tags, which are not stored; reads, recovered;
+ *     rejected_length, rejected_empty (a candidate is counted once, under the first test it fails);
+ *   - d_read_tag (may be NULL): per stored slot, the tag index of a read (also >= max_tags), -1 for a slot that is not a
+ *     candidate, -2 for a rejected candidate.  Slots that are not stored are not written.
+ * h is in the matched filter's boxcar-sum units (ntaps samples), so 10*log10(peak_power / ntaps^2) is the reply's power
+ * in dB relative to a full-scale sample. */
+typedef struct rfid_b200_report_params {
+  int32_t check_length; /* 0 or 1; 1 */
+  int32_t reserved[7];
+} rfid_b200_report_params;
+
+typedef struct rfid_b200_tag { /* 64 bytes */
+  uint8_t epc[16];                /* PC + EPC + CRC-16: the key */
+  int32_t reads, recovered;       /* reads; those whose bits came from a RECOVERED fix */
+  int32_t first_slot, last_slot;  /* slot indices s * max_windows + k */
+  int32_t peak_slot;              /* read with the largest p (rule above) */
+  float peak_power;               /* its p, boxcar-sum units squared */
+  float last_h_re, last_h_im;     /* channel estimate of the last read */
+  int64_t first_time, last_time;  /* raw samples (rule above) */
+} rfid_b200_tag;
+
+typedef struct rfid_b200_tag_summary { /* 32 bytes */
+  int32_t n_tags;                 /* all tags, also beyond max_tags */
+  int32_t reads, recovered;
+  int32_t rejected_length, rejected_empty;
+  int32_t reserved[3];
+} rfid_b200_tag_summary;
+
+RFID_B200_API void rfid_b200_default_report_params(rfid_b200_report_params* rp);
+
+/* The report of the stored slots of a decode_capture call (device pointers, asynchronous on `stream` except when the
+ * context's scratch has to grow, which synchronises): d_segs the segment table it decoded, d_results / d_counts its
+ * records and counts, d_quality its rfid_b200_window_quality records (NULL: no EMPTY rejection), d_fix its
+ * rfid_b200_recover_epc records (NULL: no recovered reads); rp NULL = defaults.  Tag j < max_tags goes to d_tags[j]; the
+ * summary to *d_summary.  Returns RFID_B200_EINVAL for a NULL ctx, segs, results, counts or summary, d_tags NULL with
+ * max_tags > 0, a negative nseg, max_windows or max_tags, nseg * max_windows >= 2^31, and check_length not 0 or 1.  A
+ * thread per slot inserts the keys into an open-addressing table (warp-aggregated), then a scan over the slots numbers
+ * the tags. */
+RFID_B200_API int rfid_b200_tag_report(rfid_b200_ctx* ctx, const rfid_b200_segment* d_segs,
+                                       const rfid_b200_window_result* d_results, const int32_t* d_counts, int nseg,
+                                       int max_windows, const rfid_b200_quality* d_quality,
+                                       const rfid_b200_epc_fix* d_fix, const rfid_b200_report_params* rp, int max_tags,
+                                       rfid_b200_tag* d_tags, rfid_b200_tag_summary* d_summary, int32_t* d_read_tag,
+                                       void* stream);
+
 /* ---------------- block mode (GNU Radio drop-in) ----------------
  * Called from the thin host blocks' general_work(); HOST pointers, owned by the
  * scheduler, touched only during the call.  State lives in the context (device
