@@ -161,6 +161,34 @@ assert TAG_DTYPE.itemsize == C.sizeof(Tag) == 64 and TAG_SUMMARY_DTYPE.itemsize 
 assert C.sizeof(ReportParams) == 32
 
 
+MATCH_ALREADY_READ, MATCH_MATCHED, MATCH_AMBIGUOUS, MATCH_NO_MATCH, MATCH_SKIPPED, MATCH_NOT_EPC = range(6)
+#: largest dictionary rfid_b200_match_epc accepts
+MATCH_MAX_DICT = 1 << 24
+
+
+class MatchParams(C.Structure):
+    """rfid_b200_match_params (include/rfid_b200.h): largest cost and smallest margin, in mean reliabilities."""
+    _fields_ = [("max_cost", C.c_float), ("min_margin", C.c_float), ("reserved", C.c_int32 * 6)]
+
+
+class EpcMatch(C.Structure):
+    _fields_ = [("status", C.c_int32), ("entry", C.c_int32), ("cost", C.c_int32), ("runner_up", C.c_int32),
+                ("n_diff", C.c_int32), ("reserved", C.c_int32 * 3)]
+
+
+class MatchCount(C.Structure):
+    _fields_ = [("matched", C.c_int32), ("first_slot", C.c_int32), ("last_slot", C.c_int32), ("reserved", C.c_int32)]
+
+
+#: numpy view of rfid_b200_epc_match (32 bytes): RFID_B200_MATCH_* status, entry, cost D1, runner-up D2, n_diff
+EPC_MATCH_DTYPE = np.dtype([("status", "<i4"), ("entry", "<i4"), ("cost", "<i4"), ("runner_up", "<i4"),
+                            ("n_diff", "<i4"), ("reserved", "<i4", (3,))])
+#: numpy view of rfid_b200_match_count (16 bytes): one dictionary entry's MATCHED windows
+MATCH_COUNT_DTYPE = np.dtype([("matched", "<i4"), ("first_slot", "<i4"), ("last_slot", "<i4"), ("reserved", "<i4")])
+assert EPC_MATCH_DTYPE.itemsize == C.sizeof(EpcMatch) == 32 and MATCH_COUNT_DTYPE.itemsize == C.sizeof(MatchCount) == 16
+assert C.sizeof(MatchParams) == 32
+
+
 def make_segments(offsets, lengths):
     segs = np.zeros(len(offsets), dtype=SEGMENT_DTYPE)
     segs["offset"] = np.asarray(offsets, dtype=np.uint64)

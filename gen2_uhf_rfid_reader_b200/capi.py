@@ -117,6 +117,10 @@ def load_library():
     L.rfid_b200_tag_report.restype = C.c_int
     L.rfid_b200_tag_report.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, vp, vp, C.POINTER(abi.ReportParams), C.c_int,
                                        vp, vp, vp, vp]
+    L.rfid_b200_default_match_params.argtypes = [C.POINTER(abi.MatchParams)]
+    L.rfid_b200_match_epc.restype = C.c_int
+    L.rfid_b200_match_epc.argtypes = [vp, vp, vp, vp, vp, C.c_int, C.c_int, vp, vp, C.c_int,
+                                      C.POINTER(abi.MatchParams), vp, vp, vp]
     _lib = L
     return L
 
@@ -133,7 +137,7 @@ EXPORTED_SYMBOLS = [
     "rfid_b200_default_cmd_params", "rfid_b200_decode_commands", "rfid_b200_decode_commands_sc16",
     "rfid_b200_decode_commands_host", "rfid_b200_default_quality_params", "rfid_b200_window_quality",
     "rfid_b200_default_recover_params", "rfid_b200_recover_epc", "rfid_b200_default_report_params",
-    "rfid_b200_tag_report",
+    "rfid_b200_tag_report", "rfid_b200_default_match_params", "rfid_b200_match_epc",
 ]
 
 
@@ -197,6 +201,15 @@ def default_report_params(**kw):
     for k, v in kw.items():
         setattr(rp, k, type(getattr(rp, k))(v))
     return rp
+
+
+def default_match_params(**kw):
+    """rfid_b200_match_params with the library's defaults (max_cost 12, min_margin 4), fields set by kw."""
+    mp = abi.MatchParams()
+    load_library().rfid_b200_default_match_params(C.byref(mp))
+    for k, v in kw.items():
+        setattr(mp, k, type(getattr(mp, k))(v))
+    return mp
 
 
 def default_params(**kw):
@@ -447,6 +460,70 @@ class Gen2Rx:
                                                   quality=quality if reject_empty else None, fixes=fixes,
                                                   params=report_params, max_tags=max_tags)
         return results, counts, quality, fixes, tags, summary, read_tag
+
+    # ---------------------------------------------------------------- capture mode: replies from tags you already know
+    def match_epc(self, windows, results, counts, dictionary, max_windows, fixes=None, n_dict=None, params=None,
+                  match=None, match_count=None, counts_per_entry=True, stream=None):
+        """Attribution records (rule: include/rfid_b200.h) of the stored windows of a `decode_capture` call: windows,
+        results and counts as in `window_quality`, fixes its `recover_epc` records (None: only CRC passes are already
+        read); dictionary: uint8 [max_dict, 16] PC + EPC + CRC frames (a CUDA tensor, or host data copied to the device);
+        n_dict: a CUDA int32 tensor whose first element is the live entry count (None: all max_dict); params:
+        `MatchParams` (None: defaults, see `default_match_params`).  Asynchronous on `stream`.  Returns (match uint8
+        [nseg * max_windows, 32], match_count uint8 [max_dict, 16] or None without counts_per_entry) as CUDA tensors;
+        `matches_to_numpy` views them.  Match records of slots beyond a segment's stored records are left as they were
+        (zero when allocated here)."""
+        import torch
+        nseg = counts.numel()
+        dev = results.device
+        if windows.numel() * windows.element_size() < nseg * max_windows * self.len_epc * 8:
+            raise ValueError("the window tap holds fewer than nseg * max_windows * len_epc complex samples")
+        if not isinstance(dictionary, torch.Tensor):
+            dictionary = torch.from_numpy(np.ascontiguousarray(dictionary, dtype=np.uint8).reshape(-1, 16)).to(dev)
+        if dictionary.dtype != torch.uint8 or not dictionary.is_contiguous() or dictionary.numel() % 16:
+            raise ValueError("the dictionary is a contiguous uint8 tensor of 16-byte frames")
+        if dictionary.data_ptr() % 16:
+            raise ValueError("the dictionary must be 16-byte aligned")
+        max_dict = dictionary.numel() // 16
+        if n_dict is not None and (n_dict.dtype != torch.int32 or n_dict.numel() < 1):
+            raise ValueError("n_dict is a CUDA int32 tensor")
+        if match is None:
+            match = torch.zeros((nseg * max_windows, 32), dtype=torch.uint8, device=dev)
+        if match_count is None and counts_per_entry:
+            match_count = torch.empty((max_dict, 16), dtype=torch.uint8, device=dev)
+        s = stream if stream is not None else torch.cuda.current_stream(dev)
+        mp = C.byref(params) if params is not None else None
+        rc = self.lib.rfid_b200_match_epc(self.h, windows.data_ptr(), results.data_ptr(), counts.data_ptr(),
+                                          fixes.data_ptr() if fixes is not None else None, nseg, max_windows,
+                                          dictionary.data_ptr() if max_dict > 0 else None,
+                                          n_dict.data_ptr() if n_dict is not None else None, max_dict, mp,
+                                          match.data_ptr(),
+                                          match_count.data_ptr() if match_count is not None and max_dict > 0 else None,
+                                          s.cuda_stream)
+        self._ck(rc, "rfid_b200_match_epc")
+        return match, match_count
+
+    def decode_capture_match(self, iq, segs, dictionary=None, max_windows=2, recover=True, reject_empty=True,
+                             quality_params=None, recover_params=None, report_params=None, match_params=None,
+                             max_tags=1024, scale=SC16_SCALE):
+        """`decode_capture_report` (decode with the window tap, quality, recovery unless recover=False, the report), then
+        `match_epc` on the same windows; iq, segs and scale as in `decode_capture` (fc32 or sc16).  dictionary None: the
+        report's own tags -- their frames are copied on the device and the report's n_tags is the live count, so the
+        call stays asynchronous.  Returns (results, counts, quality, fixes, tags, summary, read_tag, match, match_count)
+        as device tensors (fixes None without recovery)."""
+        import torch
+        tap, results, counts = self._decode_tapped(iq, segs, max_windows, scale)
+        quality = self.window_quality(tap, results, counts, max_windows, params=quality_params)
+        fixes = self.recover_epc(tap, results, counts, quality, max_windows, params=recover_params) if recover else None
+        tags, summary, read_tag = self.tag_report(results, counts, segs, max_windows,
+                                                  quality=quality if reject_empty else None, fixes=fixes,
+                                                  params=report_params, max_tags=max_tags)
+        n_dict = None
+        if dictionary is None:
+            dictionary = tags[:, :16].contiguous()
+            n_dict = summary.view(torch.int32)[:1]
+        match, match_count = self.match_epc(tap, results, counts, dictionary, max_windows, fixes=fixes, n_dict=n_dict,
+                                            params=match_params)
+        return results, counts, quality, fixes, tags, summary, read_tag, match, match_count
 
     # ---------------------------------------------------------------- capture ingest
     def segment_capture(self, iq, segmenter=None, capacity=None, stream=None, scale=SC16_SCALE):
@@ -700,13 +777,33 @@ TAG_TABLE_DTYPE = np.dtype([("epc", "U32"), ("reads", "<i4"), ("recovered", "<i4
                             ("last_us", "<f8"), ("peak_rssi_db", "<f8"), ("last_phase_deg", "<f8")])
 
 
-def tag_table(tags, ntaps=25, adc_rate=2_000_000):
+def matches_to_numpy(match, counts, max_windows, match_count=None):
+    """`match_epc` output -> (EPC_MATCH_DTYPE[nseg, max_windows], MATCH_COUNT_DTYPE[max_dict] or None)"""
+    m = match.cpu().numpy().reshape(-1).view(abi.EPC_MATCH_DTYPE).reshape(counts.numel(), max_windows)
+    mc = match_count.cpu().numpy().reshape(-1).view(abi.MATCH_COUNT_DTYPE) if match_count is not None else None
+    return m, mc
+
+
+def tag_table(tags, ntaps=25, adc_rate=2_000_000, matched=None):
     """The report's tags (TAG_DTYPE rows) in display units (host numpy only): PC + EPC + CRC as hex, reads, recovered,
     first and last seen in microseconds from the capture's first sample (the times are raw samples at adc_rate),
     peak_rssi_db = 10 log10(peak_power / ntaps^2), the strongest reply's power in dB relative to a full-scale sample (h
-    is a sum over the matched filter's ntaps samples), and last_phase_deg = arg(last h) in degrees."""
+    is a sum over the matched filter's ntaps samples), and last_phase_deg = arg(last h) in degrees.  matched: per tag,
+    the failing replies `match_epc` attributed to it (e.g. `match_count["matched"]` of a match against the report's
+    own tags); given, the table gains a `matched` column after `recovered`."""
     tags = np.asarray(tags, dtype=abi.TAG_DTYPE)
-    out = np.zeros(tags.size, dtype=TAG_TABLE_DTYPE)
+    if matched is not None:
+        matched = np.asarray(matched).reshape(-1)
+        if matched.size < tags.size:
+            raise ValueError("matched holds fewer entries than there are tags")
+        names = TAG_TABLE_DTYPE.names
+        i = names.index("recovered") + 1
+        dt = np.dtype([(n, TAG_TABLE_DTYPE[n]) for n in names[:i]] + [("matched", "<i4")] +
+                      [(n, TAG_TABLE_DTYPE[n]) for n in names[i:]])
+        out = np.zeros(tags.size, dtype=dt)
+        out["matched"] = matched[:tags.size]
+    else:
+        out = np.zeros(tags.size, dtype=TAG_TABLE_DTYPE)
     out["epc"] = [bytes(bytearray(e)).hex() for e in tags["epc"]]
     out["reads"], out["recovered"] = tags["reads"], tags["recovered"]
     out["first_us"] = tags["first_time"] * 1e6 / adc_rate

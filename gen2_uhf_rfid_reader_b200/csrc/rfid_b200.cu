@@ -20,6 +20,7 @@
 #include "rx_ingest.cuh"
 #include "rx_pack.cuh"
 #include "rx_quality.cuh"
+#include "rx_match.cuh"
 #include "rx_recover.cuh"
 #include "rx_report.cuh"
 #include "tx_synth.cuh"
@@ -84,6 +85,8 @@ struct rfid_b200_ctx {
   void* d_cmd; size_t d_cmd_bytes;
   // tag report scratch: aggregates, hash table, per-slot owners, block counts
   void* d_report; size_t d_report_bytes;
+  // EPC match scratch: row count, compact rows of the attempted windows
+  void* d_match; size_t d_match_bytes;
 };
 
 namespace {
@@ -416,6 +419,7 @@ int rfid_b200_create(const rfid_b200_params* p, rfid_b200_ctx** out)
   ctx->d_script_bytes = ctx->d_sim_res_bytes = ctx->d_sim_cnt_bytes = 0;
   ctx->d_cmd = nullptr; ctx->d_cmd_bytes = 0;
   ctx->d_report = nullptr; ctx->d_report_bytes = 0;
+  ctx->d_match = nullptr; ctx->d_match_bytes = 0;
   ctx->h_stage[0] = ctx->h_stage[1] = nullptr; ctx->ev_stage[0] = ctx->ev_stage[1] = nullptr;
   memset(&ctx->layout, 0, sizeof(ctx->layout));
   memset(&ctx->layout_sc16, 0, sizeof(ctx->layout_sc16));
@@ -504,7 +508,7 @@ void rfid_b200_destroy(rfid_b200_ctx* ctx)
   if (ctx->h_blk) cudaFreeHost(ctx->h_blk);
   void* ptrs[] = {ctx->d_blk, ctx->d_win, ctx->d_yhist, ctx->d_iq, ctx->d_segs, ctx->d_res, ctx->d_cnt, ctx->d_in, ctx->d_out, ctx->d_m2, ctx->d_mf,
                   ctx->d_gate, ctx->d_gate_out, ctx->d_one, ctx->d_mask, ctx->d_chunk, ctx->d_bursts, ctx->d_ing,
-                  ctx->d_script, ctx->d_sim_res, ctx->d_sim_cnt, ctx->d_cmd, ctx->d_report};
+                  ctx->d_script, ctx->d_sim_res, ctx->d_sim_cnt, ctx->d_cmd, ctx->d_report, ctx->d_match};
   for (void* p : ptrs)
     if (p) cudaFree(p);
   for (int b = 0; b < 2; b++) {
@@ -1491,6 +1495,65 @@ int rfid_b200_tag_report(rfid_b200_ctx* ctx, const rfid_b200_segment* d_segs, co
   if (d_read_tag) {
     rx_report_write_kernel<<<n_blocks, kReportThreads, 0, st>>>(A, true);
     launches++;
+  }
+  CK(cudaGetLastError());
+  ctx->last_launches = launches;
+  return RFID_B200_OK;
+}
+
+// ------------------------------------------------------------------ capture mode: EPC replies from tags you already know
+void rfid_b200_default_match_params(rfid_b200_match_params* mp)
+{
+  if (!mp) return;
+  memset(mp, 0, sizeof(*mp));
+  mp->max_cost = 12.0f;    // DESIGN.md 4.9: below every noise window at K = 65,536, above the weak replies' costs
+  mp->min_margin = 4.0f;
+}
+
+int rfid_b200_match_epc(rfid_b200_ctx* ctx, const float* d_windows, const rfid_b200_window_result* d_results,
+                        const int32_t* d_counts, const rfid_b200_epc_fix* d_fix, int nseg, int max_windows,
+                        const uint8_t* d_dict, const int32_t* d_n_dict, int max_dict, const rfid_b200_match_params* mp,
+                        rfid_b200_epc_match* d_match, rfid_b200_match_count* d_count, void* stream)
+{
+  if (!ctx || !d_windows || !d_results || !d_counts || !d_match || (!d_dict && max_dict > 0) || nseg < 0 ||
+      max_windows < 0 || max_dict < 0 || max_dict > kMatchMaxDict || ((uintptr_t)d_dict & 15u))
+    return RFID_B200_EINVAL;
+  const long long slots = (long long)nseg * max_windows;
+  if (slots >= (1ll << 31)) return RFID_B200_EINVAL;
+  rfid_b200_match_params d;
+  rfid_b200_default_match_params(&d);
+  if (mp) d = *mp;
+  if (!std::isfinite(d.max_cost) || !std::isfinite(d.min_margin) || d.max_cost < 0.0f || d.min_margin < 0.0f)
+    return RFID_B200_EINVAL;
+  ctx->last_launches = 0;
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  MatchArgs A;
+  A.windows = reinterpret_cast<const float2*>(d_windows);
+  A.results = d_results; A.counts = d_counts; A.fix = d_fix;
+  A.dict = reinterpret_cast<const uint4*>(d_dict); A.n_dict = d_n_dict;
+  A.match = d_match; A.match_count = d_count;
+  A.nseg = nseg; A.max_windows = max_windows; A.max_dict = max_dict;
+  A.max_cost16 = (double)d.max_cost * 16.0;
+  A.min_margin16 = (double)d.min_margin * 16.0;
+  A.cfg = ctx->cfg;
+  int launches = 0;
+  if (d_count && max_dict > 0) {
+    rx_match_init_kernel<<<(unsigned)((max_dict + 255) / 256), 256, 0, st>>>(A);
+    launches++;
+  }
+  if (slots > 0) {
+    // scratch: row count | rows [slots] (every attempted window is a row)
+    const size_t need = 256 + (size_t)slots * sizeof(MatchRow);
+    int rc;
+    if ((rc = grow(ctx, &ctx->d_match, &ctx->d_match_bytes, need))) return rc;
+    char* base = static_cast<char*>(ctx->d_match);
+    A.n_rows = reinterpret_cast<int32_t*>(base);
+    A.rows = reinterpret_cast<MatchRow*>(base + 256);
+    CK(cudaMemsetAsync(A.n_rows, 0, sizeof(int32_t), st));
+    rx_match_prepare_kernel<<<(unsigned)((slots + kMatchPrepWarps - 1) / kMatchPrepWarps), 32 * kMatchPrepWarps, 0, st>>>(A);
+    rx_match_score_kernel<<<(unsigned)((slots + kMatchRows - 1) / kMatchRows), 32 * kMatchWarps, 0, st>>>(A);
+    launches += 2;
   }
   CK(cudaGetLastError());
   ctx->last_launches = launches;

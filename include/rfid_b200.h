@@ -591,6 +591,97 @@ RFID_B200_API int rfid_b200_tag_report(rfid_b200_ctx* ctx, const rfid_b200_segme
                                        rfid_b200_tag* d_tags, rfid_b200_tag_summary* d_summary, int32_t* d_read_tag,
                                        void* stream);
 
+/* ---------------- capture mode: EPC replies from tags you already know ----------------
+ * A failing EPC window need not be decoded from scratch when the tag population is known (tags read earlier, or a
+ * manifest): it only has to be attributed to one of K known frames, maximum-likelihood decoding over a small codebook,
+ * which works far below the point where flipping a few signs (rfid_b200_recover_epc) does.  rfid_b200_match_epc scores
+ * every failing EPC window of a decode_capture call against a dictionary d_dict[k], k < K, of 16-byte PC + EPC + CRC
+ * frames (an entry need not pass its CRC); K = min(max(*d_n_dict, 0), max_dict), or max_dict when d_n_dict is NULL.
+ * Per stored slot i = s * max_windows + k, k < min(max(count[s], 0), max_windows):
+ *   1. an RN16 window (kind != EPC): NOT_EPC;
+ *   2. an EPC window with crc_ok == 1, or, with d_fix given, whose fix has status RFID_B200_FIX_RECOVERED: ALREADY_READ;
+ *   3. otherwise the window is attempted.  It is SKIPPED when crc_ok != 0 (the decoder made no EPC decisions), or when
+ *      S1 = sum of |r_j| (double, the quality rule's lane order) is 0 or not finite, with r_j, j = 0..127, the
+ *      projections exactly as the quality rule computes them.  Else, with m = S1 / 128 (double):
+ *      - reliability q_j = min(127, rint(|r_j| * 16 / m)) in double (16 steps per mean reliability, capped near 8x it);
+ *      - signs s_j = (r_j > 0); entry k's signs c_kj = c_k,j-1 xor bit_kj (frame bit j, MSB first), c_k,-1 = 1: the
+ *        signs the decoder's FM0 rule turns into that frame;
+ *      - cost D_k = sum over j of q_j * [s_j != c_kj], an exact integer (= A + sum u_j c_kj, A = sum q_j s_j,
+ *        u_j = q_j (1 - 2 s_j): the int8 product the kernel computes);
+ *      - k* = argmin D_k, ties to the lowest k; D1 = D_k*; D2 = the second smallest value of the multiset {D_k} (a
+ *        duplicate entry gives D2 = D1), INT32_MAX when K = 1;
+ *      - MATCHED iff D1 <= max_cost16 and D2 - D1 >= min_margin16; AMBIGUOUS iff only the first holds; else NO_MATCH.
+ *        The thresholds are (double)max_cost * 16 and (double)min_margin * 16 of the float parameters, compared with
+ *        the integers converted to double (the convention of the quality thresholds);
+ *      - K = 0: NO_MATCH, entry -1, cost = runner_up = INT32_MAX, n_diff -1.
+ *   Record: status, entry = k* (-1 unless a cost was computed), cost = D1, runner_up = D2, n_diff = the number of j with
+ *   s_j != c_k*j; a window that is not attempted, or SKIPPED, has entry = cost = runner_up = n_diff = -1.
+ *   Per entry k < max_dict (d_count, may be NULL; every entry is initialised by the call): matched = the MATCHED windows
+ *   naming k, first_slot / last_slot = their smallest and largest slot, -1 when there are none.
+ * Every result is an integer, a min or a max, so the bytes do not depend on launch geometry or order.  Costs are in
+ * sixteenths of the window's mean reliability (D / 16 "mean reliabilities").
+ * False attribution -- a match is an attribution under a closed-population assumption, not a CRC-verified read, which
+ * is why rfid_b200_tag_report does not count it:
+ *   - pure noise: the best of K random frames comes closer as K grows.  The smallest D1 / 16 measured (DESIGN.md 4.9)
+ *     was 31.1 / 27.1 / 20.8 at K = 16 / 1,024 / 65,536 over 10^5 Gaussian windows, and 39.1 / 30.4 / 27.6 over the
+ *     EPC windows of 612 empty simulated slots: none comes within 8 units of max_cost 12 at K = 65,536.  Larger
+ *     dictionaries lower this floor further; keep K no larger than the population can be;
+ *   - a tag outside the dictionary: two valid frames with the same PC length field can be as little as 4 sign positions
+ *     apart (e.g. frames that differ in bits 110, 111, 114, 115, 121, 122, 126, 127).  A reply from an unlisted tag that
+ *     close to a listed one is MATCHED to it at any useful max_cost.  With the replying tag held out and one CRC-valid
+ *     decoy at sign distance w from it in a 1,024-entry dictionary, the simulated weak replies were MATCHED to the decoy
+ *     in over 99 % of trials for w <= 7, in 40-45 % at w = 12 and under 1 % at w = 16 (62-64 % over w = 4..16,
+ *     DESIGN.md 4.9).  Against 1,024 random frames with the tag held out, none was MATCHED.
+ * Defaults (DESIGN.md 4.9): max_cost 12, min_margin 4. */
+enum {
+  RFID_B200_MATCH_ALREADY_READ = 0,
+  RFID_B200_MATCH_MATCHED = 1,
+  RFID_B200_MATCH_AMBIGUOUS = 2,
+  RFID_B200_MATCH_NO_MATCH = 3,
+  RFID_B200_MATCH_SKIPPED = 4,
+  RFID_B200_MATCH_NOT_EPC = 5
+};
+
+typedef struct rfid_b200_match_params {
+  float max_cost;      /* finite, >= 0, mean reliabilities; 12 */
+  float min_margin;    /* finite, >= 0, mean reliabilities; 4 */
+  int32_t reserved[6];
+} rfid_b200_match_params;
+
+/* One window's attribution (32 bytes), at the index of its window record. */
+typedef struct rfid_b200_epc_match {
+  int32_t status;      /* RFID_B200_MATCH_* */
+  int32_t entry;       /* k*, or -1 */
+  int32_t cost;        /* D1, sixteenths of the mean reliability */
+  int32_t runner_up;   /* D2 */
+  int32_t n_diff;      /* sign disagreements with entry k* */
+  int32_t reserved[3];
+} rfid_b200_epc_match;
+
+/* One dictionary entry's MATCHED windows (16 bytes). */
+typedef struct rfid_b200_match_count {
+  int32_t matched;
+  int32_t first_slot, last_slot;   /* -1 when nothing matched */
+  int32_t reserved;
+} rfid_b200_match_count;
+
+RFID_B200_API void rfid_b200_default_match_params(rfid_b200_match_params* mp);
+
+/* Attribution records of the stored windows of a decode_capture call (device pointers, asynchronous on `stream` except
+ * when the context's scratch has to grow, which synchronises): d_windows / d_results / d_counts as for
+ * rfid_b200_window_quality, d_fix its rfid_b200_recover_epc records (may be NULL), d_dict max_dict frames of 16 bytes
+ * (16-byte aligned), d_n_dict (may be NULL) the live count on the device.  Record k of segment s goes to
+ * d_match[s * max_windows + k] for k < min(d_counts[s], max_windows); nothing else is written; d_count (may be NULL)
+ * gets max_dict entries.  mp NULL = defaults.  Returns RFID_B200_EINVAL for a NULL ctx, windows, results, counts or
+ * match, d_dict NULL with max_dict > 0 or not 16-byte aligned, negative nseg, max_windows or max_dict, nseg *
+ * max_windows >= 2^31, max_dict > 2^24, and a non-finite or negative max_cost or min_margin.  One warp per slot prepares the attempted windows; the
+ * scores are an int8 tensor-core product with a fused top-2. */
+RFID_B200_API int rfid_b200_match_epc(rfid_b200_ctx* ctx, const float* d_windows, const rfid_b200_window_result* d_results,
+                                      const int32_t* d_counts, const rfid_b200_epc_fix* d_fix, int nseg, int max_windows,
+                                      const uint8_t* d_dict, const int32_t* d_n_dict, int max_dict,
+                                      const rfid_b200_match_params* mp, rfid_b200_epc_match* d_match,
+                                      rfid_b200_match_count* d_count, void* stream);
+
 /* ---------------- block mode (GNU Radio drop-in) ----------------
  * Called from the thin host blocks' general_work(); HOST pointers, owned by the
  * scheduler, touched only during the call.  State lives in the context (device
