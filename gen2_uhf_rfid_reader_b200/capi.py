@@ -43,181 +43,140 @@ def load_library():
         raise RfidB200Error("librfid_b200.so is missing: run `python -m gen2_uhf_rfid_reader_b200.build` "
                             "(there is no CPU fallback)")
     L = C.CDLL(path)
-    vp, ip, fp = C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_float)
-    L.rfid_b200_abi_version.restype = C.c_int
-    L.rfid_b200_strerror.restype = C.c_char_p
-    L.rfid_b200_strerror.argtypes = [C.c_int]
-    L.rfid_b200_last_cuda_error.restype = C.c_char_p
-    L.rfid_b200_last_cuda_error.argtypes = [vp]
-    L.rfid_b200_default_params.argtypes = [C.POINTER(abi.Params)]
-    L.rfid_b200_create.restype = C.c_int
-    L.rfid_b200_create.argtypes = [C.POINTER(abi.Params), C.POINTER(vp)]
-    L.rfid_b200_destroy.argtypes = [vp]
-    L.rfid_b200_window_length.restype = C.c_int
-    L.rfid_b200_window_length.argtypes = [vp, C.c_int]
-    L.rfid_b200_fs_dec.restype = C.c_int
-    L.rfid_b200_fs_dec.argtypes = [vp]
-    L.rfid_b200_decode_capture.restype = C.c_int
-    L.rfid_b200_decode_capture.argtypes = [vp, vp, C.c_size_t, vp, C.c_int, C.c_int, vp, vp, vp]
-    L.rfid_b200_decode_capture_sc16.restype = C.c_int
-    L.rfid_b200_decode_capture_sc16.argtypes = [vp, vp, C.c_size_t, C.c_float, vp, C.c_int, C.c_int, vp, vp, vp]
-    L.rfid_b200_decode_capture_host.restype = C.c_int
-    L.rfid_b200_decode_capture_host.argtypes = [vp, vp, C.c_size_t, vp, C.c_int, C.c_int, vp, vp]
-    L.rfid_b200_last_launch_count.restype = C.c_int
-    L.rfid_b200_last_launch_count.argtypes = [vp]
-    L.rfid_b200_kernel_time.restype = C.c_int
-    L.rfid_b200_kernel_time.argtypes = [vp, C.c_int, fp, ip]
-    L.rfid_b200_enable_kernel_timing.restype = C.c_int
-    L.rfid_b200_enable_kernel_timing.argtypes = [vp, C.c_int]
-    L.rfid_b200_set_window_tap.restype = C.c_int
-    L.rfid_b200_set_window_tap.argtypes = [vp, vp]
-    L.rfid_b200_reduce_stats.restype = C.c_int
-    L.rfid_b200_reduce_stats.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.POINTER(abi.Stats)]
-    L.rfid_b200_gate_work.restype = C.c_int
-    L.rfid_b200_gate_work.argtypes = [vp, C.c_int, vp, C.c_int, vp, C.c_int, ip, ip, ip, vp]
-    L.rfid_b200_decoder_work.restype = C.c_int
-    L.rfid_b200_decoder_work.argtypes = [vp, C.c_int, vp, C.c_int, vp, vp]
-    L.rfid_b200_mf_work.restype = C.c_int
-    L.rfid_b200_mf_work.argtypes = [vp, vp, C.c_int, vp, C.c_int, ip]
-    L.rfid_b200_default_segmenter.argtypes = [C.POINTER(abi.Segmenter)]
-    L.rfid_b200_segment_capture.restype = C.c_int
-    L.rfid_b200_segment_capture.argtypes = [vp, vp, C.c_size_t, C.POINTER(abi.Segmenter), vp, C.c_int, ip, vp]
-    L.rfid_b200_segment_capture_sc16.restype = C.c_int
-    L.rfid_b200_segment_capture_sc16.argtypes = [vp, vp, C.c_size_t, C.c_float, C.POINTER(abi.Segmenter), vp, C.c_int, ip,
-                                                 vp]
-    L.rfid_b200_ingest_capture_host_sc16.restype = C.c_int
-    L.rfid_b200_ingest_capture_host_sc16.argtypes = [vp, vp, C.c_size_t, C.c_float, C.POINTER(abi.Segmenter), C.c_int, vp,
-                                                     C.c_int, ip, vp, vp]
-    L.rfid_b200_ingest_capture_host.restype = C.c_int
-    L.rfid_b200_ingest_capture_host.argtypes = [vp, vp, C.c_size_t, C.POINTER(abi.Segmenter), C.c_int, vp, C.c_int, ip,
-                                                vp, vp]
-    L.rfid_b200_tx_synth.restype = C.c_int
-    L.rfid_b200_tx_synth.argtypes = [vp, vp, C.c_int, C.c_int, vp, C.c_size_t, C.POINTER(C.c_size_t), vp]
-    L.rfid_b200_default_sim.argtypes = [C.POINTER(abi.SimParams)]
-    L.rfid_b200_sim_segment_length.restype = C.c_int
-    L.rfid_b200_sim_segment_length.argtypes = [vp, C.POINTER(abi.SimParams)]
-    L.rfid_b200_sim_capture.restype = C.c_int
-    L.rfid_b200_sim_capture.argtypes = [vp, C.POINTER(abi.SimParams), C.c_int64, C.c_int, vp, vp, vp, vp]
-    L.rfid_b200_default_cmd_params.argtypes = [C.POINTER(abi.CmdParams)]
-    L.rfid_b200_decode_commands.restype = C.c_int
-    L.rfid_b200_decode_commands.argtypes = [vp, vp, C.c_size_t, vp, C.c_int, C.POINTER(abi.CmdParams), C.c_int, vp, vp, vp]
-    L.rfid_b200_decode_commands_sc16.restype = C.c_int
-    L.rfid_b200_decode_commands_sc16.argtypes = [vp, vp, C.c_size_t, C.c_float, vp, C.c_int, C.POINTER(abi.CmdParams),
-                                                 C.c_int, vp, vp, vp]
-    L.rfid_b200_decode_commands_host.restype = C.c_int
-    L.rfid_b200_decode_commands_host.argtypes = [vp, vp, C.c_size_t, vp, C.c_int, C.POINTER(abi.CmdParams), C.c_int, vp,
-                                                 vp]
-    L.rfid_b200_default_quality_params.argtypes = [C.POINTER(abi.QualityParams)]
-    L.rfid_b200_window_quality.restype = C.c_int
-    L.rfid_b200_window_quality.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.POINTER(abi.QualityParams), vp, vp]
-    L.rfid_b200_default_recover_params.argtypes = [C.POINTER(abi.RecoverParams)]
-    L.rfid_b200_recover_epc.restype = C.c_int
-    L.rfid_b200_recover_epc.argtypes = [vp, vp, vp, vp, vp, C.c_int, C.c_int, C.POINTER(abi.RecoverParams), vp, vp]
-    L.rfid_b200_default_report_params.argtypes = [C.POINTER(abi.ReportParams)]
-    L.rfid_b200_tag_report.restype = C.c_int
-    L.rfid_b200_tag_report.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, vp, vp, C.POINTER(abi.ReportParams), C.c_int,
-                                       vp, vp, vp, vp]
-    L.rfid_b200_default_match_params.argtypes = [C.POINTER(abi.MatchParams)]
-    L.rfid_b200_match_epc.restype = C.c_int
-    L.rfid_b200_match_epc.argtypes = [vp, vp, vp, vp, vp, C.c_int, C.c_int, vp, vp, C.c_int,
-                                      C.POINTER(abi.MatchParams), vp, vp, vp]
+    for name, (restype, argtypes) in _SIGNATURES.items():
+        f = getattr(L, name)
+        f.restype, f.argtypes = restype, argtypes
     _lib = L
     return L
 
 
-EXPORTED_SYMBOLS = [
-    "rfid_b200_abi_version", "rfid_b200_strerror", "rfid_b200_last_cuda_error", "rfid_b200_default_params",
-    "rfid_b200_create", "rfid_b200_destroy", "rfid_b200_window_length", "rfid_b200_fs_dec",
-    "rfid_b200_decode_capture", "rfid_b200_decode_capture_host", "rfid_b200_last_launch_count",
-    "rfid_b200_kernel_time", "rfid_b200_enable_kernel_timing", "rfid_b200_set_window_tap",
-    "rfid_b200_reduce_stats", "rfid_b200_gate_work", "rfid_b200_decoder_work", "rfid_b200_mf_work",
-    "rfid_b200_default_segmenter", "rfid_b200_segment_capture", "rfid_b200_ingest_capture_host",
-    "rfid_b200_tx_synth", "rfid_b200_default_sim", "rfid_b200_sim_segment_length", "rfid_b200_sim_capture",
-    "rfid_b200_decode_capture_sc16", "rfid_b200_segment_capture_sc16", "rfid_b200_ingest_capture_host_sc16",
-    "rfid_b200_default_cmd_params", "rfid_b200_decode_commands", "rfid_b200_decode_commands_sc16",
-    "rfid_b200_decode_commands_host", "rfid_b200_default_quality_params", "rfid_b200_window_quality",
-    "rfid_b200_default_recover_params", "rfid_b200_recover_epc", "rfid_b200_default_report_params",
-    "rfid_b200_tag_report", "rfid_b200_default_match_params", "rfid_b200_match_epc",
-]
+_vp, _int, _size, _float = C.c_void_p, C.c_int, C.c_size_t, C.c_float
+_ip, _P = C.POINTER(C.c_int), C.POINTER
+# Every function include/rfid_b200.h declares: name -> (restype, argtypes).  The void functions keep ctypes' default
+# restype, c_int.
+_SIGNATURES = {
+    "rfid_b200_abi_version": (_int, []),
+    "rfid_b200_strerror": (C.c_char_p, [_int]),
+    "rfid_b200_last_cuda_error": (C.c_char_p, [_vp]),
+    "rfid_b200_default_params": (_int, [_P(abi.Params)]),
+    "rfid_b200_create": (_int, [_P(abi.Params), _P(_vp)]),
+    "rfid_b200_destroy": (_int, [_vp]),
+    "rfid_b200_window_length": (_int, [_vp, _int]),
+    "rfid_b200_fs_dec": (_int, [_vp]),
+    "rfid_b200_decode_capture": (_int, [_vp, _vp, _size, _vp, _int, _int, _vp, _vp, _vp]),
+    "rfid_b200_decode_capture_sc16": (_int, [_vp, _vp, _size, _float, _vp, _int, _int, _vp, _vp, _vp]),
+    "rfid_b200_decode_capture_host": (_int, [_vp, _vp, _size, _vp, _int, _int, _vp, _vp]),
+    "rfid_b200_last_launch_count": (_int, [_vp]),
+    "rfid_b200_kernel_time": (_int, [_vp, _int, _P(_float), _ip]),
+    "rfid_b200_enable_kernel_timing": (_int, [_vp, _int]),
+    "rfid_b200_set_window_tap": (_int, [_vp, _vp]),
+    "rfid_b200_reduce_stats": (_int, [_vp, _vp, _vp, _int, _int, _int, _P(abi.Stats)]),
+    "rfid_b200_gate_work": (_int, [_vp, _int, _vp, _int, _vp, _int, _ip, _ip, _ip, _vp]),
+    "rfid_b200_decoder_work": (_int, [_vp, _int, _vp, _int, _vp, _vp]),
+    "rfid_b200_mf_work": (_int, [_vp, _vp, _int, _vp, _int, _ip]),
+    "rfid_b200_default_segmenter": (_int, [_P(abi.Segmenter)]),
+    "rfid_b200_segment_capture": (_int, [_vp, _vp, _size, _P(abi.Segmenter), _vp, _int, _ip, _vp]),
+    "rfid_b200_segment_capture_sc16": (_int, [_vp, _vp, _size, _float, _P(abi.Segmenter), _vp, _int, _ip, _vp]),
+    "rfid_b200_ingest_capture_host": (_int, [_vp, _vp, _size, _P(abi.Segmenter), _int, _vp, _int, _ip, _vp, _vp]),
+    "rfid_b200_ingest_capture_host_sc16": (_int, [_vp, _vp, _size, _float, _P(abi.Segmenter), _int, _vp, _int, _ip, _vp,
+                                                  _vp]),
+    "rfid_b200_tx_synth": (_int, [_vp, _vp, _int, _int, _vp, _size, _P(_size), _vp]),
+    "rfid_b200_default_sim": (_int, [_P(abi.SimParams)]),
+    "rfid_b200_sim_segment_length": (_int, [_vp, _P(abi.SimParams)]),
+    "rfid_b200_sim_capture": (_int, [_vp, _P(abi.SimParams), C.c_int64, _int, _vp, _vp, _vp, _vp]),
+    "rfid_b200_default_cmd_params": (_int, [_P(abi.CmdParams)]),
+    "rfid_b200_decode_commands": (_int, [_vp, _vp, _size, _vp, _int, _P(abi.CmdParams), _int, _vp, _vp, _vp]),
+    "rfid_b200_decode_commands_sc16": (_int, [_vp, _vp, _size, _float, _vp, _int, _P(abi.CmdParams), _int, _vp, _vp,
+                                              _vp]),
+    "rfid_b200_decode_commands_host": (_int, [_vp, _vp, _size, _vp, _int, _P(abi.CmdParams), _int, _vp, _vp]),
+    "rfid_b200_default_quality_params": (_int, [_P(abi.QualityParams)]),
+    "rfid_b200_window_quality": (_int, [_vp, _vp, _vp, _vp, _int, _int, _P(abi.QualityParams), _vp, _vp]),
+    "rfid_b200_default_recover_params": (_int, [_P(abi.RecoverParams)]),
+    "rfid_b200_recover_epc": (_int, [_vp, _vp, _vp, _vp, _vp, _int, _int, _P(abi.RecoverParams), _vp, _vp]),
+    "rfid_b200_default_report_params": (_int, [_P(abi.ReportParams)]),
+    "rfid_b200_tag_report": (_int, [_vp, _vp, _vp, _vp, _int, _int, _vp, _vp, _P(abi.ReportParams), _int, _vp, _vp, _vp,
+                                    _vp]),
+    "rfid_b200_default_match_params": (_int, [_P(abi.MatchParams)]),
+    "rfid_b200_match_epc": (_int, [_vp, _vp, _vp, _vp, _vp, _int, _int, _vp, _vp, _int, _P(abi.MatchParams), _vp, _vp,
+                                   _vp]),
+}
+EXPORTED_SYMBOLS = list(_SIGNATURES)
 
 
-def _sc16_samples(iq):
-    """complex samples of an int16 capture shaped (2n,) or (n, 2) (interleaved I, Q: UHD's sc16)"""
+def _capture(iq, scale):
+    """(entry-point suffix, leading arguments) of a CUDA capture: ("", (pointer, samples)) for complex64 or float32
+    interleaved (fc32), ("_sc16", (pointer, samples, scale)) for a torch.int16 tensor shaped (2n,) or (n, 2) holding
+    interleaved I, Q (UHD's sc16)"""
+    import torch
+    if iq.dtype != torch.int16:
+        return "", (iq.data_ptr(), iq.numel() if iq.is_complex() else iq.numel() // 2)
     if iq.dim() == 2 and iq.shape[1] != 2 or iq.dim() > 2 or iq.numel() % 2:
         raise ValueError("an int16 capture is shaped (2n,) or (n, 2): interleaved I, Q")
     if not iq.is_contiguous():
         raise ValueError("an int16 capture must be contiguous")
-    return iq.numel() // 2
+    return "_sc16", (iq.data_ptr(), iq.numel() // 2, scale)
 
 
-def default_sim(**kw):
-    p = abi.SimParams()
-    load_library().rfid_b200_default_sim(C.byref(p))
+def _stream(stream, device):
+    """the CUDA handle of `stream`, or of the current torch stream on `device`"""
+    import torch
+    return (stream if stream is not None else torch.cuda.current_stream(device)).cuda_stream
+
+
+def _ptr(t):
+    return t.data_ptr() if t is not None else None
+
+
+def _ref(params):
+    return C.byref(params) if params is not None else None
+
+
+def _defaults(struct, fill, kw, cast=None):
+    """`struct` filled by the library's `fill`, then the fields in kw set (converted by cast, by default to the
+    field's type)"""
+    p = struct()
+    getattr(load_library(), fill)(C.byref(p))
     for k, v in kw.items():
-        setattr(p, k, type(getattr(p, k))(v))
+        setattr(p, k, (cast or type(getattr(p, k)))(v))
     return p
 
 
+def default_sim(**kw):
+    return _defaults(abi.SimParams, "rfid_b200_default_sim", kw)
+
+
 def default_segmenter(**kw):
-    sp = abi.Segmenter()
-    load_library().rfid_b200_default_segmenter(C.byref(sp))
-    for k, v in kw.items():
-        setattr(sp, k, type(getattr(sp, k))(v))
-    return sp
+    return _defaults(abi.Segmenter, "rfid_b200_default_segmenter", kw)
 
 
 def default_cmd_params(**kw):
     """rfid_b200_cmd_params with the library's defaults (level_frac 0.5, level_abs 0, gap_us 400), fields set by kw."""
-    cp = abi.CmdParams()
-    load_library().rfid_b200_default_cmd_params(C.byref(cp))
-    for k, v in kw.items():
-        setattr(cp, k, type(getattr(cp, k))(v))
-    return cp
+    return _defaults(abi.CmdParams, "rfid_b200_default_cmd_params", kw)
 
 
 def default_quality_params(**kw):
     """rfid_b200_quality_params with the library's defaults (empty_db 9.5, single_snr_db 8.8), fields set by kw."""
-    qp = abi.QualityParams()
-    load_library().rfid_b200_default_quality_params(C.byref(qp))
-    for k, v in kw.items():
-        setattr(qp, k, type(getattr(qp, k))(v))
-    return qp
+    return _defaults(abi.QualityParams, "rfid_b200_default_quality_params", kw)
 
 
 def default_recover_params(**kw):
     """rfid_b200_recover_params with the library's defaults (positions 12, max_flips 4, min_snr_db 7.0), fields set by
     kw."""
-    rp = abi.RecoverParams()
-    load_library().rfid_b200_default_recover_params(C.byref(rp))
-    for k, v in kw.items():
-        setattr(rp, k, type(getattr(rp, k))(v))
-    return rp
+    return _defaults(abi.RecoverParams, "rfid_b200_default_recover_params", kw)
 
 
 def default_report_params(**kw):
     """rfid_b200_report_params with the library's defaults (check_length 1), fields set by kw."""
-    rp = abi.ReportParams()
-    load_library().rfid_b200_default_report_params(C.byref(rp))
-    for k, v in kw.items():
-        setattr(rp, k, type(getattr(rp, k))(v))
-    return rp
+    return _defaults(abi.ReportParams, "rfid_b200_default_report_params", kw)
 
 
 def default_match_params(**kw):
     """rfid_b200_match_params with the library's defaults (max_cost 12, min_margin 4), fields set by kw."""
-    mp = abi.MatchParams()
-    load_library().rfid_b200_default_match_params(C.byref(mp))
-    for k, v in kw.items():
-        setattr(mp, k, type(getattr(mp, k))(v))
-    return mp
+    return _defaults(abi.MatchParams, "rfid_b200_default_match_params", kw)
 
 
 def default_params(**kw):
-    p = abi.Params()
-    load_library().rfid_b200_default_params(C.byref(p))
-    for k, v in kw.items():
-        setattr(p, k, int(v))
-    return p
+    return _defaults(abi.Params, "rfid_b200_default_params", kw, int)
 
 
 class Gen2Rx:
@@ -256,6 +215,14 @@ class Gen2Rx:
             raise RfidB200Error("%s: %s (%s)" % (what, self.lib.rfid_b200_strerror(rc).decode(),
                                                  self.lib.rfid_b200_last_cuda_error(self.h).decode()))
 
+    def _call(self, name, *args):
+        """lib.name(context, *args), raising on an error code"""
+        self._ck(getattr(self.lib, name)(self.h, *args), name)
+
+    def _check_tap(self, windows, nseg, max_windows):
+        if windows.numel() * windows.element_size() < nseg * max_windows * self.len_epc * 8:
+            raise ValueError("the window tap holds fewer than nseg * max_windows * len_epc complex samples")
+
     # ---------------------------------------------------------------- capture mode
     def decode_capture(self, iq, segs, max_windows=4, results=None, counts=None, stream=None, scale=SC16_SCALE):
         """iq: CUDA complex64 (or float32 interleaved) tensor, or a torch.int16 tensor shaped (2n,) or (n, 2) holding an
@@ -264,21 +231,13 @@ class Gen2Rx:
         `stream` (default: the current torch stream).  Returns (results uint8[nseg*max_windows,64], counts int32[nseg])."""
         import torch
         nseg = segs.numel() * segs.element_size() // 16
-        sc16 = iq.dtype == torch.int16
-        n_raw = _sc16_samples(iq) if sc16 else (iq.numel() if iq.is_complex() else iq.numel() // 2)
+        fmt, cap = _capture(iq, scale)
         if results is None:
             results = torch.zeros((nseg * max_windows, 64), dtype=torch.uint8, device=iq.device)
         if counts is None:
             counts = torch.zeros(nseg, dtype=torch.int32, device=iq.device)
-        s = stream if stream is not None else torch.cuda.current_stream(iq.device)
-        if sc16:
-            rc = self.lib.rfid_b200_decode_capture_sc16(self.h, iq.data_ptr(), n_raw, scale, segs.data_ptr(), nseg,
-                                                        max_windows, results.data_ptr(), counts.data_ptr(), s.cuda_stream)
-            self._ck(rc, "rfid_b200_decode_capture_sc16")
-            return results, counts
-        rc = self.lib.rfid_b200_decode_capture(self.h, iq.data_ptr(), n_raw, segs.data_ptr(), nseg, max_windows,
-                                               results.data_ptr(), counts.data_ptr(), s.cuda_stream)
-        self._ck(rc, "rfid_b200_decode_capture")
+        self._call("rfid_b200_decode_capture" + fmt, *cap, segs.data_ptr(), nseg, max_windows, results.data_ptr(),
+                   counts.data_ptr(), _stream(stream, iq.device))
         return results, counts
 
     def decode_capture_host(self, iq, segs, max_windows=4):
@@ -288,15 +247,13 @@ class Gen2Rx:
         nseg = segs.size
         recs = np.zeros((nseg, max_windows), dtype=abi.RESULT_DTYPE)
         counts = np.zeros(nseg, dtype=np.int32)
-        rc = self.lib.rfid_b200_decode_capture_host(self.h, raw.ctypes.data, raw.size // 2, segs.ctypes.data, nseg,
-                                                    max_windows, recs.ctypes.data, counts.ctypes.data)
-        self._ck(rc, "rfid_b200_decode_capture_host")
+        self._call("rfid_b200_decode_capture_host", raw.ctypes.data, raw.size // 2, segs.ctypes.data, nseg, max_windows,
+                   recs.ctypes.data, counts.ctypes.data)
         return recs, counts
 
     def decode_capture_host_ptr(self, iq_ptr, n_raw, segs_ptr, nseg, max_windows, res_ptr, cnt_ptr):
         """Same call on raw (e.g. pinned) host pointers: no Python-side copies."""
-        rc = self.lib.rfid_b200_decode_capture_host(self.h, iq_ptr, n_raw, segs_ptr, nseg, max_windows, res_ptr, cnt_ptr)
-        self._ck(rc, "rfid_b200_decode_capture_host")
+        self._call("rfid_b200_decode_capture_host", iq_ptr, n_raw, segs_ptr, nseg, max_windows, res_ptr, cnt_ptr)
 
     # ---------------------------------------------------------------- capture mode: the reader's commands
     def decode_commands(self, iq, segs, max_commands=8, commands=None, counts=None, stream=None, scale=SC16_SCALE,
@@ -307,23 +264,13 @@ class Gen2Rx:
         counts int32[nseg]); `commands_to_numpy` views them as COMMAND_DTYPE."""
         import torch
         nseg = segs.numel() * segs.element_size() // 16
-        sc16 = iq.dtype == torch.int16
-        n_raw = _sc16_samples(iq) if sc16 else (iq.numel() if iq.is_complex() else iq.numel() // 2)
+        fmt, cap = _capture(iq, scale)
         if commands is None:
             commands = torch.zeros((nseg * max_commands, 64), dtype=torch.uint8, device=iq.device)
         if counts is None:
             counts = torch.zeros(nseg, dtype=torch.int32, device=iq.device)
-        s = stream if stream is not None else torch.cuda.current_stream(iq.device)
-        cp = C.byref(params) if params is not None else None
-        if sc16:
-            rc = self.lib.rfid_b200_decode_commands_sc16(self.h, iq.data_ptr(), n_raw, scale, segs.data_ptr(), nseg, cp,
-                                                         max_commands, commands.data_ptr(), counts.data_ptr(),
-                                                         s.cuda_stream)
-            self._ck(rc, "rfid_b200_decode_commands_sc16")
-        else:
-            rc = self.lib.rfid_b200_decode_commands(self.h, iq.data_ptr(), n_raw, segs.data_ptr(), nseg, cp, max_commands,
-                                                    commands.data_ptr(), counts.data_ptr(), s.cuda_stream)
-            self._ck(rc, "rfid_b200_decode_commands")
+        self._call("rfid_b200_decode_commands" + fmt, *cap, segs.data_ptr(), nseg, _ref(params), max_commands,
+                   commands.data_ptr(), counts.data_ptr(), _stream(stream, iq.device))
         return commands, counts
 
     def decode_commands_host(self, iq, segs, max_commands=8, params=None):
@@ -334,11 +281,8 @@ class Gen2Rx:
         nseg = segs.size
         cmds = np.zeros((nseg, max_commands), dtype=abi.COMMAND_DTYPE)
         counts = np.zeros(nseg, dtype=np.int32)
-        cp = C.byref(params) if params is not None else None
-        rc = self.lib.rfid_b200_decode_commands_host(self.h, raw.ctypes.data, raw.size // 2, segs.ctypes.data, nseg, cp,
-                                                     max_commands, cmds.ctypes.data if cmds.size else None,
-                                                     counts.ctypes.data)
-        self._ck(rc, "rfid_b200_decode_commands_host")
+        self._call("rfid_b200_decode_commands_host", raw.ctypes.data, raw.size // 2, segs.ctypes.data, nseg,
+                   _ref(params), max_commands, cmds.ctypes.data if cmds.size else None, counts.ctypes.data)
         return cmds, counts
 
     # ---------------------------------------------------------------- capture mode: reply quality and slot outcome
@@ -350,15 +294,11 @@ class Gen2Rx:
         slots beyond a segment's stored records are left as they were (zero when allocated here)."""
         import torch
         nseg = counts.numel()
-        if windows.numel() * windows.element_size() < nseg * max_windows * self.len_epc * 8:
-            raise ValueError("the window tap holds fewer than nseg * max_windows * len_epc complex samples")
+        self._check_tap(windows, nseg, max_windows)
         if quality is None:
             quality = torch.zeros((nseg * max_windows, 16), dtype=torch.uint8, device=results.device)
-        s = stream if stream is not None else torch.cuda.current_stream(results.device)
-        qp = C.byref(params) if params is not None else None
-        rc = self.lib.rfid_b200_window_quality(self.h, windows.data_ptr(), results.data_ptr(), counts.data_ptr(), nseg,
-                                               max_windows, qp, quality.data_ptr(), s.cuda_stream)
-        self._ck(rc, "rfid_b200_window_quality")
+        self._call("rfid_b200_window_quality", windows.data_ptr(), results.data_ptr(), counts.data_ptr(), nseg,
+                   max_windows, _ref(params), quality.data_ptr(), _stream(stream, results.device))
         return quality
 
     def decode_capture_quality(self, iq, segs, max_windows=2, params=None, scale=SC16_SCALE):
@@ -367,8 +307,7 @@ class Gen2Rx:
         device memory (3.5 GB for 160,000 segments of 2 windows at 2 MS/s); it is released to torch's stream-ordered
         allocator on return, so the call stays asynchronous on the current stream like `decode_capture`.  Returns
         (results, counts, quality) as device tensors."""
-        tap, results, counts = self._decode_tapped(iq, segs, max_windows, scale)
-        return results, counts, self.window_quality(tap, results, counts, max_windows, params=params)
+        return self._decode_stages(iq, segs, max_windows, scale, params)[1][:3]
 
     def _decode_tapped(self, iq, segs, max_windows, scale):
         """`decode_capture` with a window tap set for this one call: (tap, results, counts)"""
@@ -382,6 +321,20 @@ class Gen2Rx:
             self.set_window_tap(None)
         return tap, results, counts
 
+    def _decode_stages(self, iq, segs, max_windows, scale, quality_params, recover=False, recover_params=None,
+                       report=False, reject_empty=True, report_params=None, max_tags=1024):
+        """`_decode_tapped`, then `window_quality`, `recover_epc` (recover) and `tag_report` (report) on what they
+        wrote: (tap, (results, counts, quality, fixes, tags, summary, read_tag)), None for what a stage not run would
+        give"""
+        tap, results, counts = self._decode_tapped(iq, segs, max_windows, scale)
+        quality = self.window_quality(tap, results, counts, max_windows, params=quality_params)
+        fixes = self.recover_epc(tap, results, counts, quality, max_windows, params=recover_params) if recover else None
+        tags = (None, None, None)
+        if report:
+            tags = self.tag_report(results, counts, segs, max_windows, quality=quality if reject_empty else None,
+                                   fixes=fixes, params=report_params, max_tags=max_tags)
+        return tap, (results, counts, quality, fixes) + tags
+
     # ---------------------------------------------------------------- capture mode: EPC replies that fail their CRC
     def recover_epc(self, windows, results, counts, quality, max_windows, params=None, fixes=None, stream=None):
         """Recovery records (rule: include/rfid_b200.h) of the stored windows of a `decode_capture` call: windows, results
@@ -391,15 +344,12 @@ class Gen2Rx:
         (zero when allocated here).  `apply_fixes` folds the RECOVERED windows into the records."""
         import torch
         nseg = counts.numel()
-        if windows.numel() * windows.element_size() < nseg * max_windows * self.len_epc * 8:
-            raise ValueError("the window tap holds fewer than nseg * max_windows * len_epc complex samples")
+        self._check_tap(windows, nseg, max_windows)
         if fixes is None:
             fixes = torch.zeros((nseg * max_windows, 32), dtype=torch.uint8, device=results.device)
-        s = stream if stream is not None else torch.cuda.current_stream(results.device)
-        rp = C.byref(params) if params is not None else None
-        rc = self.lib.rfid_b200_recover_epc(self.h, windows.data_ptr(), results.data_ptr(), counts.data_ptr(),
-                                            quality.data_ptr(), nseg, max_windows, rp, fixes.data_ptr(), s.cuda_stream)
-        self._ck(rc, "rfid_b200_recover_epc")
+        self._call("rfid_b200_recover_epc", windows.data_ptr(), results.data_ptr(), counts.data_ptr(),
+                   quality.data_ptr(), nseg, max_windows, _ref(params), fixes.data_ptr(),
+                   _stream(stream, results.device))
         return fixes
 
     def decode_capture_recover(self, iq, segs, max_windows=2, quality_params=None, recover_params=None,
@@ -407,10 +357,7 @@ class Gen2Rx:
         """`decode_capture` with the window tap set for this one call, then `window_quality` and `recover_epc` on what it
         wrote; iq, segs and scale as in `decode_capture` (fc32 or sc16), the tap as in `decode_capture_quality`.
         Returns (results, counts, quality, fixes) as device tensors; the records are the decoder's, unchanged."""
-        tap, results, counts = self._decode_tapped(iq, segs, max_windows, scale)
-        quality = self.window_quality(tap, results, counts, max_windows, params=quality_params)
-        fixes = self.recover_epc(tap, results, counts, quality, max_windows, params=recover_params)
-        return results, counts, quality, fixes
+        return self._decode_stages(iq, segs, max_windows, scale, quality_params, True, recover_params)[1][:4]
 
     # ---------------------------------------------------------------- capture mode: the tag inventory report
     def tag_report(self, results, counts, segs, max_windows, quality=None, fixes=None, params=None, max_tags=1024,
@@ -435,14 +382,9 @@ class Gen2Rx:
             summary = torch.zeros(32, dtype=torch.uint8, device=dev)
         if read_tag is None:
             read_tag = torch.full((nseg * max_windows,), -1, dtype=torch.int32, device=dev)
-        s = stream if stream is not None else torch.cuda.current_stream(dev)
-        rp = C.byref(params) if params is not None else None
-        rc = self.lib.rfid_b200_tag_report(self.h, segs.data_ptr(), results.data_ptr(), counts.data_ptr(), nseg,
-                                           max_windows, quality.data_ptr() if quality is not None else None,
-                                           fixes.data_ptr() if fixes is not None else None, rp, max_tags,
-                                           tags.data_ptr() if max_tags > 0 else None, summary.data_ptr(),
-                                           read_tag.data_ptr(), s.cuda_stream)
-        self._ck(rc, "rfid_b200_tag_report")
+        self._call("rfid_b200_tag_report", segs.data_ptr(), results.data_ptr(), counts.data_ptr(), nseg, max_windows,
+                   _ptr(quality), _ptr(fixes), _ref(params), max_tags, tags.data_ptr() if max_tags > 0 else None,
+                   summary.data_ptr(), read_tag.data_ptr(), _stream(stream, dev))
         return tags, summary, read_tag
 
     def decode_capture_report(self, iq, segs, max_windows=2, recover=True, reject_empty=True, quality_params=None,
@@ -453,13 +395,8 @@ class Gen2Rx:
         passes on noise; but also replies weaker than quality_params.empty_db, DESIGN 4.8).  Only the report has to
         come back to the host.  Returns (results, counts, quality, fixes, tags, summary, read_tag) as device tensors
         (fixes None without recovery)."""
-        tap, results, counts = self._decode_tapped(iq, segs, max_windows, scale)
-        quality = self.window_quality(tap, results, counts, max_windows, params=quality_params)
-        fixes = self.recover_epc(tap, results, counts, quality, max_windows, params=recover_params) if recover else None
-        tags, summary, read_tag = self.tag_report(results, counts, segs, max_windows,
-                                                  quality=quality if reject_empty else None, fixes=fixes,
-                                                  params=report_params, max_tags=max_tags)
-        return results, counts, quality, fixes, tags, summary, read_tag
+        return self._decode_stages(iq, segs, max_windows, scale, quality_params, recover, recover_params, report=True,
+                                   reject_empty=reject_empty, report_params=report_params, max_tags=max_tags)[1]
 
     # ---------------------------------------------------------------- capture mode: replies from tags you already know
     def match_epc(self, windows, results, counts, dictionary, max_windows, fixes=None, n_dict=None, params=None,
@@ -475,8 +412,7 @@ class Gen2Rx:
         import torch
         nseg = counts.numel()
         dev = results.device
-        if windows.numel() * windows.element_size() < nseg * max_windows * self.len_epc * 8:
-            raise ValueError("the window tap holds fewer than nseg * max_windows * len_epc complex samples")
+        self._check_tap(windows, nseg, max_windows)
         if not isinstance(dictionary, torch.Tensor):
             dictionary = torch.from_numpy(np.ascontiguousarray(dictionary, dtype=np.uint8).reshape(-1, 16)).to(dev)
         if dictionary.dtype != torch.uint8 or not dictionary.is_contiguous() or dictionary.numel() % 16:
@@ -490,16 +426,9 @@ class Gen2Rx:
             match = torch.zeros((nseg * max_windows, 32), dtype=torch.uint8, device=dev)
         if match_count is None and counts_per_entry:
             match_count = torch.empty((max_dict, 16), dtype=torch.uint8, device=dev)
-        s = stream if stream is not None else torch.cuda.current_stream(dev)
-        mp = C.byref(params) if params is not None else None
-        rc = self.lib.rfid_b200_match_epc(self.h, windows.data_ptr(), results.data_ptr(), counts.data_ptr(),
-                                          fixes.data_ptr() if fixes is not None else None, nseg, max_windows,
-                                          dictionary.data_ptr() if max_dict > 0 else None,
-                                          n_dict.data_ptr() if n_dict is not None else None, max_dict, mp,
-                                          match.data_ptr(),
-                                          match_count.data_ptr() if match_count is not None and max_dict > 0 else None,
-                                          s.cuda_stream)
-        self._ck(rc, "rfid_b200_match_epc")
+        self._call("rfid_b200_match_epc", windows.data_ptr(), results.data_ptr(), counts.data_ptr(), _ptr(fixes), nseg,
+                   max_windows, dictionary.data_ptr() if max_dict > 0 else None, _ptr(n_dict), max_dict, _ref(params),
+                   match.data_ptr(), _ptr(match_count) if max_dict > 0 else None, _stream(stream, dev))
         return match, match_count
 
     def decode_capture_match(self, iq, segs, dictionary=None, max_windows=2, recover=True, reject_empty=True,
@@ -511,40 +440,27 @@ class Gen2Rx:
         call stays asynchronous.  Returns (results, counts, quality, fixes, tags, summary, read_tag, match, match_count)
         as device tensors (fixes None without recovery)."""
         import torch
-        tap, results, counts = self._decode_tapped(iq, segs, max_windows, scale)
-        quality = self.window_quality(tap, results, counts, max_windows, params=quality_params)
-        fixes = self.recover_epc(tap, results, counts, quality, max_windows, params=recover_params) if recover else None
-        tags, summary, read_tag = self.tag_report(results, counts, segs, max_windows,
-                                                  quality=quality if reject_empty else None, fixes=fixes,
-                                                  params=report_params, max_tags=max_tags)
+        tap, out = self._decode_stages(iq, segs, max_windows, scale, quality_params, recover, recover_params,
+                                       report=True, reject_empty=reject_empty, report_params=report_params,
+                                       max_tags=max_tags)
+        results, counts, _, fixes, tags, summary, _ = out
         n_dict = None
         if dictionary is None:
             dictionary = tags[:, :16].contiguous()
             n_dict = summary.view(torch.int32)[:1]
-        match, match_count = self.match_epc(tap, results, counts, dictionary, max_windows, fixes=fixes, n_dict=n_dict,
-                                            params=match_params)
-        return results, counts, quality, fixes, tags, summary, read_tag, match, match_count
+        return out + self.match_epc(tap, results, counts, dictionary, max_windows, fixes=fixes, n_dict=n_dict,
+                                    params=match_params)
 
     # ---------------------------------------------------------------- capture ingest
     def segment_capture(self, iq, segmenter=None, capacity=None, stream=None, scale=SC16_SCALE):
         """CW-gap segment table (SEGMENT_DTYPE ndarray) of a CUDA capture tensor (complex64 / float32 interleaved, or an
         sc16 torch.int16 tensor as in `decode_capture`, whose table is that of its conversion)."""
-        import torch
-        sc16 = iq.dtype == torch.int16
-        n_raw = _sc16_samples(iq) if sc16 else (iq.numel() if iq.is_complex() else iq.numel() // 2)
-        cap = int(capacity) if capacity is not None else max(16, n_raw // 4096)
+        fmt, cap_args = _capture(iq, scale)
+        cap = int(capacity) if capacity is not None else max(16, cap_args[1] // 4096)
         segs = np.zeros(cap, dtype=abi.SEGMENT_DTYPE)
         n = C.c_int(0)
-        s = stream if stream is not None else torch.cuda.current_stream(iq.device)
-        sp = C.byref(segmenter) if segmenter else None
-        if sc16:
-            rc = self.lib.rfid_b200_segment_capture_sc16(self.h, iq.data_ptr(), n_raw, scale, sp, segs.ctypes.data, cap,
-                                                         C.byref(n), s.cuda_stream)
-            self._ck(rc, "rfid_b200_segment_capture_sc16")
-        else:
-            rc = self.lib.rfid_b200_segment_capture(self.h, iq.data_ptr(), n_raw, sp, segs.ctypes.data, cap, C.byref(n),
-                                                    s.cuda_stream)
-            self._ck(rc, "rfid_b200_segment_capture")
+        self._call("rfid_b200_segment_capture" + fmt, *cap_args, _ref(segmenter), segs.ctypes.data, cap, C.byref(n),
+                   _stream(stream, iq.device))
         return segs[:n.value].copy()
 
     def ingest_capture_host(self, iq, segmenter=None, max_windows=4, capacity=None, scale=SC16_SCALE):
@@ -561,16 +477,9 @@ class Gen2Rx:
         recs = np.zeros((cap, max_windows), dtype=abi.RESULT_DTYPE)
         counts = np.zeros(cap, dtype=np.int32)
         n = C.c_int(0)
-        sp = C.byref(segmenter) if segmenter else None
-        if sc16:
-            rc = self.lib.rfid_b200_ingest_capture_host_sc16(self.h, raw.ctypes.data, n_raw, scale, sp, max_windows,
-                                                             segs.ctypes.data, cap, C.byref(n), recs.ctypes.data,
-                                                             counts.ctypes.data)
-            self._ck(rc, "rfid_b200_ingest_capture_host_sc16")
-        else:
-            rc = self.lib.rfid_b200_ingest_capture_host(self.h, raw.ctypes.data, n_raw, sp, max_windows, segs.ctypes.data,
-                                                        cap, C.byref(n), recs.ctypes.data, counts.ctypes.data)
-            self._ck(rc, "rfid_b200_ingest_capture_host")
+        head = (n_raw, scale) if sc16 else (n_raw,)
+        self._call("rfid_b200_ingest_capture_host" + ("_sc16" if sc16 else ""), raw.ctypes.data, *head, _ref(segmenter),
+                   max_windows, segs.ctypes.data, cap, C.byref(n), recs.ctypes.data, counts.ctypes.data)
         k = n.value
         return segs[:k].copy(), recs[:k].copy(), counts[:k].copy()
 
@@ -580,12 +489,10 @@ class Gen2Rx:
         import torch
         scr = np.array([(int(k), int(a)) for k, a in script], dtype=abi.TX_COMMAND_DTYPE)
         n = C.c_size_t(0)
-        self._ck(self.lib.rfid_b200_tx_synth(self.h, scr.ctypes.data, scr.size, dac_rate, None, 0, C.byref(n), None),
-                 "rfid_b200_tx_synth")
+        self._call("rfid_b200_tx_synth", scr.ctypes.data, scr.size, dac_rate, None, 0, C.byref(n), None)
         out = torch.empty(n.value, dtype=torch.float32, device=device)
-        s = torch.cuda.current_stream(out.device)
-        self._ck(self.lib.rfid_b200_tx_synth(self.h, scr.ctypes.data, scr.size, dac_rate, out.data_ptr(), out.numel(),
-                                             C.byref(n), s.cuda_stream), "rfid_b200_tx_synth")
+        self._call("rfid_b200_tx_synth", scr.ctypes.data, scr.size, dac_rate, out.data_ptr(), out.numel(), C.byref(n),
+                   _stream(None, out.device))
         return out
 
     def sim_segment_length(self, sim):
@@ -603,21 +510,19 @@ class Gen2Rx:
         iq = out if out is not None else torch.empty(nseg * seg_len, dtype=torch.complex64, device=dev)
         segs = torch.zeros((nseg, 16), dtype=torch.uint8, device=dev)
         truth = torch.zeros((nseg, 48), dtype=torch.uint8, device=dev)
-        s = torch.cuda.current_stream(dev)
-        self._ck(self.lib.rfid_b200_sim_capture(self.h, C.byref(sim), first_segment, nseg, iq.data_ptr(), segs.data_ptr(),
-                                                truth.data_ptr(), s.cuda_stream), "rfid_b200_sim_capture")
+        self._call("rfid_b200_sim_capture", C.byref(sim), first_segment, nseg, iq.data_ptr(), segs.data_ptr(),
+                   truth.data_ptr(), _stream(None, dev))
         return {"iq": iq, "segs": segs, "truth": truth, "segment_len": seg_len}
 
     def set_window_tap(self, tensor_or_none):
-        ptr = tensor_or_none.data_ptr() if tensor_or_none is not None else None
-        self._ck(self.lib.rfid_b200_set_window_tap(self.h, ptr), "rfid_b200_set_window_tap")
+        self._call("rfid_b200_set_window_tap", _ptr(tensor_or_none))
 
     def enable_kernel_timing(self, on=True):
-        self._ck(self.lib.rfid_b200_enable_kernel_timing(self.h, int(on)), "rfid_b200_enable_kernel_timing")
+        self._call("rfid_b200_enable_kernel_timing", int(on))
 
     def kernel_time(self, reset=True):
         ms, n = C.c_float(0), C.c_int(0)
-        self._ck(self.lib.rfid_b200_kernel_time(self.h, int(reset), C.byref(ms), C.byref(n)), "rfid_b200_kernel_time")
+        self._call("rfid_b200_kernel_time", int(reset), C.byref(ms), C.byref(n))
         return ms.value, n.value
 
     def last_launch_count(self):
@@ -629,8 +534,8 @@ class Gen2Rx:
         nseg = counts.size
         max_per = recs.size // nseg if nseg else 1
         st = abi.Stats()
-        self._ck(self.lib.rfid_b200_reduce_stats(self.h, recs.ctypes.data, counts.ctypes.data, nseg, max(1, max_per),
-                                                 int(bool(continuous)), C.byref(st)), "rfid_b200_reduce_stats")
+        self._call("rfid_b200_reduce_stats", recs.ctypes.data, counts.ctypes.data, nseg, max(1, max_per),
+                   int(bool(continuous)), C.byref(st))
         return st
 
     # ---------------------------------------------------------------- block mode
@@ -640,9 +545,8 @@ class Gen2Rx:
         out = np.zeros(max(n, 1), dtype=np.complex64)
         m2 = np.zeros(max(n, 1), dtype=np.float32) if want_magn2 else None
         c, w, cl = C.c_int(0), C.c_int(0), C.c_int(0)
-        rc = self.lib.rfid_b200_gate_work(self.h, int(seek), x.ctypes.data, n, out.ctypes.data, max(n, 1),
-                                          C.byref(c), C.byref(w), C.byref(cl), m2.ctypes.data if want_magn2 else None)
-        self._ck(rc, "rfid_b200_gate_work")
+        self._call("rfid_b200_gate_work", int(seek), x.ctypes.data, n, out.ctypes.data, max(n, 1), C.byref(c),
+                   C.byref(w), C.byref(cl), m2.ctypes.data if want_magn2 else None)
         res = {"consumed": c.value, "written": w.value, "closed": cl.value, "out": out[:w.value]}
         if want_magn2:
             res["magn2"] = m2[:w.value]
@@ -652,8 +556,7 @@ class Gen2Rx:
         w = np.ascontiguousarray(window, dtype=np.complex64)
         rec = np.zeros(1, dtype=abi.RESULT_DTYPE)
         bits = np.zeros(128, dtype=np.float32)
-        rc = self.lib.rfid_b200_decoder_work(self.h, int(kind), w.ctypes.data, w.size, rec.ctypes.data, bits.ctypes.data)
-        self._ck(rc, "rfid_b200_decoder_work")
+        self._call("rfid_b200_decoder_work", int(kind), w.ctypes.data, w.size, rec.ctypes.data, bits.ctypes.data)
         return rec[0], bits[:16 if kind == abi.RN16 else 128]
 
     def mf_work(self, chunk):
@@ -661,8 +564,7 @@ class Gen2Rx:
         cap = x.size // self.params.decim + 2
         out = np.zeros(cap, dtype=np.complex64)
         w = C.c_int(0)
-        rc = self.lib.rfid_b200_mf_work(self.h, x.ctypes.data, x.size, out.ctypes.data, cap, C.byref(w))
-        self._ck(rc, "rfid_b200_mf_work")
+        self._call("rfid_b200_mf_work", x.ctypes.data, x.size, out.ctypes.data, cap, C.byref(w))
         return out[:w.value]
 
 
@@ -673,18 +575,21 @@ def segments_to_device(segs, device):
     return torch.from_numpy(b.copy()).to(device)
 
 
+def _records_to_numpy(records, counts, per_segment, dtype):
+    """device uint8[nseg*per_segment,dtype.itemsize] + int32[nseg] -> (dtype[nseg,per_segment], int32[nseg])"""
+    r = records.cpu().numpy().reshape(-1).view(dtype)
+    c = counts.cpu().numpy()
+    return r.reshape(c.size, per_segment), c
+
+
 def results_to_numpy(results, counts, max_windows):
     """device uint8[nseg*max_windows,64] + int32[nseg] -> (RESULT_DTYPE[nseg,max_windows], int32[nseg])"""
-    r = results.cpu().numpy().reshape(-1).view(abi.RESULT_DTYPE)
-    c = counts.cpu().numpy()
-    return r.reshape(c.size, max_windows), c
+    return _records_to_numpy(results, counts, max_windows, abi.RESULT_DTYPE)
 
 
 def commands_to_numpy(cmds, counts, max_commands):
     """device uint8[nseg*max_commands,64] + int32[nseg] -> (COMMAND_DTYPE[nseg,max_commands], int32[nseg])"""
-    r = cmds.cpu().numpy().reshape(-1).view(abi.COMMAND_DTYPE)
-    c = counts.cpu().numpy()
-    return r.reshape(c.size, max_commands), c
+    return _records_to_numpy(cmds, counts, max_commands, abi.COMMAND_DTYPE)
 
 
 #: one row per stored tag window: the reader command that armed it (see `transcript`)
@@ -737,16 +642,12 @@ def transcript(cmds, cmd_counts, recs, counts, decim=5, adc_rate=2_000_000):
 
 def quality_to_numpy(quality, counts, max_windows):
     """device uint8[nseg*max_windows,16] + int32[nseg] -> (QUALITY_DTYPE[nseg,max_windows], int32[nseg])"""
-    q = quality.cpu().numpy().reshape(-1).view(abi.QUALITY_DTYPE)
-    c = counts.cpu().numpy()
-    return q.reshape(c.size, max_windows), c
+    return _records_to_numpy(quality, counts, max_windows, abi.QUALITY_DTYPE)
 
 
 def fixes_to_numpy(fixes, counts, max_windows):
     """device uint8[nseg*max_windows,32] + int32[nseg] -> (EPC_FIX_DTYPE[nseg,max_windows], int32[nseg])"""
-    f = fixes.cpu().numpy().reshape(-1).view(abi.EPC_FIX_DTYPE)
-    c = counts.cpu().numpy()
-    return f.reshape(c.size, max_windows), c
+    return _records_to_numpy(fixes, counts, max_windows, abi.EPC_FIX_DTYPE)
 
 
 def apply_fixes(recs, counts, fixes):
@@ -779,7 +680,7 @@ TAG_TABLE_DTYPE = np.dtype([("epc", "U32"), ("reads", "<i4"), ("recovered", "<i4
 
 def matches_to_numpy(match, counts, max_windows, match_count=None):
     """`match_epc` output -> (EPC_MATCH_DTYPE[nseg, max_windows], MATCH_COUNT_DTYPE[max_dict] or None)"""
-    m = match.cpu().numpy().reshape(-1).view(abi.EPC_MATCH_DTYPE).reshape(counts.numel(), max_windows)
+    m = _records_to_numpy(match, counts, max_windows, abi.EPC_MATCH_DTYPE)[0]
     mc = match_count.cpu().numpy().reshape(-1).view(abi.MATCH_COUNT_DTYPE) if match_count is not None else None
     return m, mc
 

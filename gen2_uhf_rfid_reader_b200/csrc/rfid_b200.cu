@@ -27,6 +27,17 @@
 
 using namespace rfid_b200;
 
+// A device buffer of the context, freed with it; grow() sizes the scratch buffers on demand.
+struct DevBuf {
+  void* p = nullptr;
+  size_t bytes = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  ~DevBuf() { if (p) cudaFree(p); }
+};
+
+// Created by value-initialisation: every member not set by rfid_b200_create starts zero.
 struct rfid_b200_ctx {
   rfid_b200_params params;
   RxConfig cfg;
@@ -41,7 +52,6 @@ struct rfid_b200_ctx {
   float* window_tap;
   int last_launches;
   bool timing;
-  cudaEvent_t ev0, ev1;
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> pending;
   std::vector<cudaEvent_t> ev_pool;  // timing events are created once and reused (no driver calls inside a timed loop)
   float kernel_ms;
@@ -50,43 +60,35 @@ struct rfid_b200_ctx {
   int pack_g_override;  // RFID_B200_PACK_G (developer aid): segments per CTA of the pack kernel, 0 = automatic
   bool pack_disabled;   // RFID_B200_KERNEL=split: keep the one-CTA-per-segment kernels for every configuration
   // host-mode staging buffers
-  void* d_iq; size_t d_iq_bytes;
-  void* d_segs; size_t d_segs_bytes;
-  void* d_res; size_t d_res_bytes;
-  void* d_cnt; size_t d_cnt_bytes;
-  void* d_win; size_t d_win_bytes;  // per-segment window scratch of the one-CTA-per-segment kernels
-  void* d_yhist;                     // rx_pack_kernel: y history, [%nsmid][kPMaxSeg][kYW] float2
+  DevBuf d_iq, d_segs, d_res, d_cnt;
+  DevBuf d_win;                      // per-segment window scratch of the one-CTA-per-segment kernels
+  DevBuf d_yhist;                    // rx_pack_kernel: y history, [%nsmid][kPMaxSeg][kYW] float2
   cudaEvent_t ev_hist;               // recorded after every rx_pack_kernel launch: the history serves one launch at a time
   cudaStream_t hist_stream;          // stream of the last rx_pack_kernel launch
   bool hist_used;
   // block mode
-  GateState* d_gate;
-  GateCallOut* d_gate_out;
-  void* d_in; size_t d_in_bytes;
-  void* d_out; size_t d_out_bytes;
-  void* d_m2; size_t d_m2_bytes;
-  void* d_blk; size_t d_blk_bytes;   // block mode: [GateCallOut | out samples | |out|^2] in one block -> ONE D2H per work call
+  DevBuf d_gate;                     // GateState
+  DevBuf d_in, d_out, d_m2;
+  DevBuf d_blk;                      // block mode: [GateCallOut | out samples | |out|^2] in one block -> ONE D2H per work call
   void* h_blk; size_t h_blk_bytes;   // its pinned host mirror
-  rfid_b200_window_result* d_one;
+  DevBuf d_one;                      // rfid_b200_window_result
   // mf block mode
-  void* d_mf; size_t d_mf_bytes; long long mf_abs0; long long mf_have; long long mf_next_n;
+  DevBuf d_mf; long long mf_abs0; long long mf_have; long long mf_next_n;
   // capture ingest (segmenter work buffers, pinned upload staging)
-  void* d_mask; size_t d_mask_bytes;
-  void* d_chunk; size_t d_chunk_bytes;  // chunk_last | prev_low | falls_before | chunk_falls
-  void* d_bursts; size_t d_bursts_bytes;
-  void* d_ing;  // level partials + totals
+  DevBuf d_mask;
+  DevBuf d_chunk;  // chunk_last | prev_low | falls_before | chunk_falls
+  DevBuf d_bursts;
+  DevBuf d_ing;    // level partials + totals
   void* h_stage[2]; cudaEvent_t ev_stage[2];
   std::vector<IngestBurst> h_bursts;
   // TX synthesiser / slot simulator
-  void* d_script; size_t d_script_bytes;
-  void* d_sim_res; size_t d_sim_res_bytes;
-  void* d_sim_cnt; size_t d_sim_cnt_bytes;
+  DevBuf d_script, d_sim_res, d_sim_cnt;
   // host-mode command records
-  void* d_cmd; size_t d_cmd_bytes;
+  DevBuf d_cmd;
   // tag report scratch: aggregates, hash table, per-slot owners, block counts
-  void* d_report; size_t d_report_bytes;
+  DevBuf d_report;
   // EPC match scratch: row count, compact rows of the attempted windows
-  void* d_match; size_t d_match_bytes;
+  DevBuf d_match;
 };
 
 namespace {
@@ -321,17 +323,20 @@ pack_fn pack_kernel(int pas, bool sc16)
   return pas == kPASMax ? rx_pack_kernel<5, 5, kPASMax, RawFc32> : rx_pack_kernel<5, 5, kPASMax - 1, RawFc32>;
 }
 
-int grow(rfid_b200_ctx* ctx, void** p, size_t* have, size_t need)
+int grow(rfid_b200_ctx* ctx, DevBuf& b, size_t need)
 {
-  if (*have >= need) return RFID_B200_OK;
-  if (*p) cudaFree(*p);
-  *p = nullptr; *have = 0;
+  if (b.bytes >= need) return RFID_B200_OK;
+  if (b.p) cudaFree(b.p);
+  b.p = nullptr; b.bytes = 0;
   size_t want = need + need / 4 + 256;
-  cudaError_t e = cudaMalloc(p, want);
+  cudaError_t e = cudaMalloc(&b.p, want);
   if (e != cudaSuccess) { ctx->last_error = "cudaMalloc failed"; cudaGetLastError(); return RFID_B200_ENOMEM; }
-  *have = want;
+  b.bytes = want;
   return RFID_B200_OK;
 }
+
+// grid of the kernels that run one warp per record slot
+unsigned slot_grid(long long slots) { return (unsigned)((slots + kSlotWarps - 1) / kSlotWarps); }
 
 // Segments per CTA of rx_pack_kernel: as few CTAs as fill the device once (one CTA per SM, every SM busy for the
 // whole launch); larger batches run kPMaxSeg per CTA in several waves.  With its decoder warps one pool over the
@@ -404,43 +409,21 @@ int rfid_b200_create(const rfid_b200_params* p, rfid_b200_ctx** out)
   rfid_b200_ctx* ctx = new (std::nothrow) rfid_b200_ctx();
   if (!ctx) return RFID_B200_ENOMEM;
   ctx->params = *p; ctx->cfg = cfg; ctx->device = p->device;
-  ctx->window_tap = nullptr; ctx->last_launches = 0; ctx->timing = false; ctx->kernel_ms = 0.f; ctx->kernel_launches = 0;
-  ctx->d_iq = ctx->d_segs = ctx->d_res = ctx->d_cnt = ctx->d_in = ctx->d_out = ctx->d_m2 = ctx->d_mf = nullptr;
-  ctx->d_win = nullptr; ctx->d_win_bytes = 0;
-  ctx->d_yhist = nullptr;
-  ctx->ev_hist = nullptr; ctx->hist_stream = nullptr; ctx->hist_used = false;
-  ctx->d_blk = nullptr; ctx->d_blk_bytes = 0; ctx->h_blk = nullptr; ctx->h_blk_bytes = 0;
-  ctx->d_iq_bytes = ctx->d_segs_bytes = ctx->d_res_bytes = ctx->d_cnt_bytes = ctx->d_in_bytes = ctx->d_out_bytes = ctx->d_m2_bytes = ctx->d_mf_bytes = 0;
-  ctx->d_gate = nullptr; ctx->d_gate_out = nullptr; ctx->d_one = nullptr;
-  ctx->mf_abs0 = 0; ctx->mf_have = 0; ctx->mf_next_n = 0;
-  ctx->d_mask = ctx->d_chunk = ctx->d_bursts = ctx->d_ing = nullptr;
-  ctx->d_mask_bytes = ctx->d_chunk_bytes = ctx->d_bursts_bytes = 0;
-  ctx->d_script = ctx->d_sim_res = ctx->d_sim_cnt = nullptr;
-  ctx->d_script_bytes = ctx->d_sim_res_bytes = ctx->d_sim_cnt_bytes = 0;
-  ctx->d_cmd = nullptr; ctx->d_cmd_bytes = 0;
-  ctx->d_report = nullptr; ctx->d_report_bytes = 0;
-  ctx->d_match = nullptr; ctx->d_match_bytes = 0;
-  ctx->h_stage[0] = ctx->h_stage[1] = nullptr; ctx->ev_stage[0] = ctx->ev_stage[1] = nullptr;
-  memset(&ctx->layout, 0, sizeof(ctx->layout));
-  memset(&ctx->layout_sc16, 0, sizeof(ctx->layout_sc16));
   make_layout(cfg, (int)sizeof(RawFc32::T), ctx->layout);
   make_layout(cfg, (int)sizeof(RawSc16::T), ctx->layout_sc16);
   cudaError_t e = cudaSetDevice(p->device);
   if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking);
-  ctx->copy_stream = nullptr;
-  for (int k = 0; k < 4; k++) ctx->ev_slice[k] = nullptr;
   if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking);
   for (int k = 0; k < 4 && e == cudaSuccess; k++) e = cudaEventCreateWithFlags(&ctx->ev_slice[k], cudaEventDisableTiming);
-  if (e == cudaSuccess) e = cudaMalloc((void**)&ctx->d_gate, sizeof(GateState));
-  if (e == cudaSuccess) e = cudaMalloc((void**)&ctx->d_gate_out, sizeof(GateCallOut));
-  if (e == cudaSuccess) e = cudaMalloc((void**)&ctx->d_one, sizeof(rfid_b200_window_result));
-  if (e == cudaSuccess) e = cudaMemsetAsync(ctx->d_gate, 0, sizeof(GateState), ctx->stream);
+  if (e == cudaSuccess) e = cudaMalloc(&ctx->d_gate.p, sizeof(GateState));
+  if (e == cudaSuccess) e = cudaMalloc(&ctx->d_one.p, sizeof(rfid_b200_window_result));
+  if (e == cudaSuccess) e = cudaMemsetAsync(ctx->d_gate.p, 0, sizeof(GateState), ctx->stream);
   if (e == cudaSuccess) {
     // gate_impl ctor (gate_impl.cc:45) + initialize_reader_state (global_vars.cc:47): NEG_EDGE, first SEEK = RN16
     GateState init;
     memset(&init, 0, sizeof(init));
     init.to_ungate = cfg.len_rn16;
-    e = cudaMemcpyAsync(ctx->d_gate, &init, offsetof(GateState, win_samples), cudaMemcpyHostToDevice, ctx->stream);
+    e = cudaMemcpyAsync(ctx->d_gate.p, &init, offsetof(GateState, win_samples), cudaMemcpyHostToDevice, ctx->stream);
   }
   if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
   ctx->sm_count = prop.multiProcessorCount;
@@ -462,7 +445,7 @@ int rfid_b200_create(const rfid_b200_params* p, rfid_b200_ctx** out)
       cudaFree(d_n);
     }
     if (e == cudaSuccess && nsmid < (unsigned)prop.multiProcessorCount) nsmid = prop.multiProcessorCount;
-    if (e == cudaSuccess) e = cudaMalloc(&ctx->d_yhist, (size_t)nsmid * kPMaxSeg * kYW * sizeof(float2));
+    if (e == cudaSuccess) e = cudaMalloc(&ctx->d_yhist.p, (size_t)nsmid * kPMaxSeg * kYW * sizeof(float2));
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->ev_hist, cudaEventDisableTiming);
   }
   if (e == cudaSuccess && pack_ok(cfg)) {
@@ -506,11 +489,6 @@ void rfid_b200_destroy(rfid_b200_ctx* ctx)
   for (cudaEvent_t e : ctx->ev_pool) cudaEventDestroy(e);
   ctx->ev_pool.clear();
   if (ctx->h_blk) cudaFreeHost(ctx->h_blk);
-  void* ptrs[] = {ctx->d_blk, ctx->d_win, ctx->d_yhist, ctx->d_iq, ctx->d_segs, ctx->d_res, ctx->d_cnt, ctx->d_in, ctx->d_out, ctx->d_m2, ctx->d_mf,
-                  ctx->d_gate, ctx->d_gate_out, ctx->d_one, ctx->d_mask, ctx->d_chunk, ctx->d_bursts, ctx->d_ing,
-                  ctx->d_script, ctx->d_sim_res, ctx->d_sim_cnt, ctx->d_cmd, ctx->d_report, ctx->d_match};
-  for (void* p : ptrs)
-    if (p) cudaFree(p);
   for (int b = 0; b < 2; b++) {
     if (ctx->h_stage[b]) cudaFreeHost(ctx->h_stage[b]);
     if (ctx->ev_stage[b]) cudaEventDestroy(ctx->ev_stage[b]);
@@ -519,7 +497,7 @@ void rfid_b200_destroy(rfid_b200_ctx* ctx)
   if (ctx->ev_hist) cudaEventDestroy(ctx->ev_hist);
   if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
   if (ctx->stream) cudaStreamDestroy(ctx->stream);
-  delete ctx;
+  delete ctx;   // (frees the device buffers)
 }
 
 int rfid_b200_window_length(const rfid_b200_ctx* ctx, int kind)
@@ -605,10 +583,10 @@ static int decode_capture_impl(rfid_b200_ctx* ctx, const void* d_iq, bool sc16, 
   if (!use_pack) {
     // window scratch: one RN16 + one EPC window per segment (grown on demand; cudaMalloc synchronises, so a
     // caller that wants a fully asynchronous call sizes the context once with its largest batch)
-    int rc = grow(ctx, &ctx->d_win, &ctx->d_win_bytes, (size_t)nseg * A.win_stride * sizeof(float2));
+    int rc = grow(ctx, ctx->d_win, (size_t)nseg * A.win_stride * sizeof(float2));
     if (rc) return rc;
   }
-  A.win_scratch = reinterpret_cast<float2*>(ctx->d_win);
+  A.win_scratch = reinterpret_cast<float2*>(ctx->d_win.p);
   A.iq = d_iq;
   A.scale = scale;
   A.n_raw = n_raw;
@@ -633,7 +611,7 @@ static int decode_capture_impl(rfid_b200_ctx* ctx, const void* d_iq, bool sc16, 
     memset(&P, 0, sizeof(P));
     make_layout_pack(ctx->cfg, pack_segments_per_cta(ctx, nseg), sc16 ? (int)sizeof(RawSc16::T) : (int)sizeof(RawFc32::T), P);
     P.iq = A.iq; P.scale = scale; P.n_raw = A.n_raw; P.segs = A.segs; P.nseg = nseg; P.seg_base = seg_base; P.max_windows = A.max_windows;
-    P.results = A.results; P.counts = A.counts; P.window_tap = A.window_tap; P.y_hist = reinterpret_cast<float2*>(ctx->d_yhist);
+    P.results = A.results; P.counts = A.counts; P.window_tap = A.window_tap; P.y_hist = reinterpret_cast<float2*>(ctx->d_yhist.p);
     P.cfg = ctx->cfg;
     // the y history belongs to one launch at a time: a launch on another stream than the previous one waits for it
     if (ctx->hist_used && ctx->hist_stream != s) CK(cudaStreamWaitEvent(s, ctx->ev_hist, 0));
@@ -662,13 +640,13 @@ int rfid_b200_decode_capture_host(rfid_b200_ctx* ctx, const float* h_iq, size_t 
   CK(cudaSetDevice(ctx->device));
   int rc;
   const size_t res_bytes = (size_t)nseg * max_windows_per_segment * sizeof(rfid_b200_window_result);
-  if ((rc = grow(ctx, &ctx->d_iq, &ctx->d_iq_bytes, n_raw * 8 + 16))) return rc;
-  if ((rc = grow(ctx, &ctx->d_segs, &ctx->d_segs_bytes, (size_t)nseg * sizeof(rfid_b200_segment)))) return rc;
-  if ((rc = grow(ctx, &ctx->d_res, &ctx->d_res_bytes, res_bytes))) return rc;
-  if ((rc = grow(ctx, &ctx->d_cnt, &ctx->d_cnt_bytes, (size_t)nseg * 4))) return rc;
+  if ((rc = grow(ctx, ctx->d_iq, n_raw * 8 + 16))) return rc;
+  if ((rc = grow(ctx, ctx->d_segs, (size_t)nseg * sizeof(rfid_b200_segment)))) return rc;
+  if ((rc = grow(ctx, ctx->d_res, res_bytes))) return rc;
+  if ((rc = grow(ctx, ctx->d_cnt, (size_t)nseg * 4))) return rc;
   cudaStream_t s = ctx->stream;
-  CK(cudaMemcpyAsync(ctx->d_segs, h_segs, (size_t)nseg * sizeof(rfid_b200_segment), cudaMemcpyHostToDevice, s));
-  CK(cudaMemsetAsync(ctx->d_res, 0, res_bytes, s));
+  CK(cudaMemcpyAsync(ctx->d_segs.p, h_segs, (size_t)nseg * sizeof(rfid_b200_segment), cudaMemcpyHostToDevice, s));
+  CK(cudaMemsetAsync(ctx->d_res.p, 0, res_bytes, s));
   // Pinned source: the call is a pipeline over slices of the segment table -- upload of slice k+1 (copy stream) beside the
   // decode of slice k and the download of slice k-1's records (compute stream).  The call as a whole is bound by the
   // host -> device link (8 B per sample); the pipeline takes the decode and the record download off its tail.
@@ -677,7 +655,7 @@ int rfid_b200_decode_capture_host(rfid_b200_ctx* ctx, const float* h_iq, size_t 
   const bool pinned = cudaPointerGetAttributes(&attr, h_iq) == cudaSuccess && attr.type == cudaMemoryTypeHost;
   cudaGetLastError();
   const int n_slices = (pinned && nseg >= 64) ? 4 : 1;
-  if (n_slices == 1) CK(cudaMemcpyAsync(ctx->d_iq, h_iq, n_raw * 8, cudaMemcpyHostToDevice, s));
+  if (n_slices == 1) CK(cudaMemcpyAsync(ctx->d_iq.p, h_iq, n_raw * 8, cudaMemcpyHostToDevice, s));
   int launches = 0;
   for (int k = 0; k < n_slices; k++) {
     const int b = (int)((long long)nseg * k / n_slices), e = (int)((long long)nseg * (k + 1) / n_slices);
@@ -692,20 +670,20 @@ int rfid_b200_decode_capture_host(rfid_b200_ctx* ctx, const float* h_iq, size_t 
       if (hi > n_raw) hi = n_raw;
       if (lo > hi) lo = hi;
       lo = lo >= 4 ? lo - 4 : 0;  // (the tile loader rounds a segment's first sample down to an even index)
-      if (hi > lo) CK(cudaMemcpyAsync((char*)ctx->d_iq + lo * 8, (const char*)h_iq + lo * 8, (hi - lo) * 8, cudaMemcpyHostToDevice, ctx->copy_stream));
+      if (hi > lo) CK(cudaMemcpyAsync((char*)ctx->d_iq.p + lo * 8, (const char*)h_iq + lo * 8, (hi - lo) * 8, cudaMemcpyHostToDevice, ctx->copy_stream));
       CK(cudaEventRecord(ctx->ev_slice[k], ctx->copy_stream));
       CK(cudaStreamWaitEvent(s, ctx->ev_slice[k], 0));
     }
-    rc = decode_capture_impl(ctx, ctx->d_iq, false, 1.f, n_raw, (const rfid_b200_segment*)ctx->d_segs + b, e - b,
-                             max_windows_per_segment, (rfid_b200_window_result*)ctx->d_res + (size_t)b * max_windows_per_segment,
-                             (int32_t*)ctx->d_cnt + b, s, b);
+    rc = decode_capture_impl(ctx, ctx->d_iq.p, false, 1.f, n_raw, (const rfid_b200_segment*)ctx->d_segs.p + b, e - b,
+                             max_windows_per_segment, (rfid_b200_window_result*)ctx->d_res.p + (size_t)b * max_windows_per_segment,
+                             (int32_t*)ctx->d_cnt.p + b, s, b);
     if (rc) return rc;
     launches += ctx->last_launches;
     const size_t rb = (size_t)(e - b) * max_windows_per_segment * sizeof(rfid_b200_window_result);
     CK(cudaMemcpyAsync((char*)h_results + (size_t)b * max_windows_per_segment * sizeof(rfid_b200_window_result),
-                       (char*)ctx->d_res + (size_t)b * max_windows_per_segment * sizeof(rfid_b200_window_result), rb,
+                       (char*)ctx->d_res.p + (size_t)b * max_windows_per_segment * sizeof(rfid_b200_window_result), rb,
                        cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(h_counts + b, (int32_t*)ctx->d_cnt + b, (size_t)(e - b) * 4, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(h_counts + b, (int32_t*)ctx->d_cnt.p + b, (size_t)(e - b) * 4, cudaMemcpyDeviceToHost, s));
   }
   CK(cudaStreamSynchronize(s));
   ctx->last_launches = launches;
@@ -810,16 +788,10 @@ int ingest_alloc(rfid_b200_ctx* ctx, size_t n_raw, const SegmenterCfg& sc, long 
   n_chunks = (long long)((n_raw + kIngestChunk - 1) / kIngestChunk);
   burst_cap = (unsigned int)(n_raw / sc.gap + 4);
   int rc;
-  if ((rc = grow(ctx, &ctx->d_mask, &ctx->d_mask_bytes, (size_t)n_chunks * 32 * 4))) return rc;
-  if ((rc = grow(ctx, &ctx->d_chunk, &ctx->d_chunk_bytes, (size_t)n_chunks * 28 + 64))) return rc;
-  if ((rc = grow(ctx, &ctx->d_bursts, &ctx->d_bursts_bytes, (size_t)burst_cap * sizeof(IngestBurst)))) return rc;
-  if (!ctx->d_ing) {
-    if (cudaMalloc(&ctx->d_ing, kLevelBlocks * sizeof(double) + sizeof(IngestTotals)) != cudaSuccess) {
-      cudaGetLastError();
-      return RFID_B200_ENOMEM;
-    }
-  }
-  return RFID_B200_OK;
+  if ((rc = grow(ctx, ctx->d_mask, (size_t)n_chunks * 32 * 4))) return rc;
+  if ((rc = grow(ctx, ctx->d_chunk, (size_t)n_chunks * 28 + 64))) return rc;
+  if ((rc = grow(ctx, ctx->d_bursts, (size_t)burst_cap * sizeof(IngestBurst)))) return rc;
+  return grow(ctx, ctx->d_ing, kLevelBlocks * sizeof(double) + sizeof(IngestTotals));
 }
 
 struct IngestPtrs {
@@ -830,10 +802,10 @@ struct IngestPtrs {
 IngestPtrs ingest_ptrs(rfid_b200_ctx* ctx, long long n_chunks)
 {
   IngestPtrs P;
-  P.partial = reinterpret_cast<double*>(ctx->d_ing);
+  P.partial = reinterpret_cast<double*>(ctx->d_ing.p);
   P.tot = reinterpret_cast<IngestTotals*>(P.partial + kLevelBlocks);
-  P.mask = reinterpret_cast<unsigned int*>(ctx->d_mask);
-  P.chunk_last = reinterpret_cast<long long*>(ctx->d_chunk);
+  P.mask = reinterpret_cast<unsigned int*>(ctx->d_mask.p);
+  P.chunk_last = reinterpret_cast<long long*>(ctx->d_chunk.p);
   P.prev_low = P.chunk_last + n_chunks;
   P.falls_before = reinterpret_cast<unsigned long long*>(P.prev_low + n_chunks);
   P.chunk_falls = reinterpret_cast<unsigned int*>(P.falls_before + n_chunks);
@@ -885,7 +857,7 @@ int finish_bursts(rfid_b200_ctx* ctx, long long n_chunks, unsigned int burst_cap
   long long blocks = (n_chunks + 7) / 8;
   if (blocks > ctx->sm_count * 8) blocks = ctx->sm_count * 8;
   ingest_bursts<<<(unsigned)blocks, 256, 0, s>>>(n_chunks, P.mask, P.prev_low, P.falls_before, sc.gap,
-                                                 reinterpret_cast<IngestBurst*>(ctx->d_bursts), burst_cap, P.tot);
+                                                 reinterpret_cast<IngestBurst*>(ctx->d_bursts.p), burst_cap, P.tot);
   CK(cudaGetLastError());
   ctx->last_launches += 2;
   CK(cudaMemcpyAsync(&tot, P.tot, sizeof(tot), cudaMemcpyDeviceToHost, s));
@@ -893,7 +865,7 @@ int finish_bursts(rfid_b200_ctx* ctx, long long n_chunks, unsigned int burst_cap
   if (tot.n_bursts > burst_cap) { ctx->last_error = "segmenter: burst list overflow"; return RFID_B200_ECAPACITY; }
   ctx->h_bursts.resize(tot.n_bursts);
   if (tot.n_bursts) {
-    CK(cudaMemcpyAsync(ctx->h_bursts.data(), ctx->d_bursts, (size_t)tot.n_bursts * sizeof(IngestBurst), cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(ctx->h_bursts.data(), ctx->d_bursts.p, (size_t)tot.n_bursts * sizeof(IngestBurst), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
   }
   std::sort(ctx->h_bursts.begin(), ctx->h_bursts.end(), [](const IngestBurst& a, const IngestBurst& b) { return a.pos < b.pos; });
@@ -992,10 +964,10 @@ static int ingest_capture_host_impl(rfid_b200_ctx* ctx, const void* h_iq, bool s
   long long n_chunks;
   unsigned int burst_cap;
   if ((rc = ingest_alloc(ctx, n_raw, sc, n_chunks, burst_cap))) return rc;
-  if ((rc = grow(ctx, &ctx->d_iq, &ctx->d_iq_bytes, n_raw * sb + 16))) return rc;
+  if ((rc = grow(ctx, ctx->d_iq, n_raw * sb + 16))) return rc;
   const IngestPtrs P = ingest_ptrs(ctx, n_chunks);
   cudaStream_t s = ctx->stream;
-  const DevCapture X{ctx->d_iq, sc16, scale};
+  const DevCapture X{ctx->d_iq.p, sc16, scale};
 
   // pageable sources go through two pinned staging slices so the host memcpy of slice k+1 overlaps the DMA of
   // slice k; pinned (registered) sources are DMA'd directly.  The threshold pass runs behind each slice.
@@ -1023,10 +995,10 @@ static int ingest_capture_host_impl(rfid_b200_ctx* ctx, const void* h_iq, bool s
       const int b = (int)(slice & 1);
       if (slice >= 2) CK(cudaEventSynchronize(ctx->ev_stage[b]));
       memcpy(ctx->h_stage[b], src, n * sb);
-      CK(cudaMemcpyAsync((char*)ctx->d_iq + off * sb, ctx->h_stage[b], n * sb, cudaMemcpyHostToDevice, s));
+      CK(cudaMemcpyAsync((char*)ctx->d_iq.p + off * sb, ctx->h_stage[b], n * sb, cudaMemcpyHostToDevice, s));
       CK(cudaEventRecord(ctx->ev_stage[b], s));
     } else {
-      CK(cudaMemcpyAsync((char*)ctx->d_iq + off * sb, src, n * sb, cudaMemcpyHostToDevice, s));
+      CK(cudaMemcpyAsync((char*)ctx->d_iq.p + off * sb, src, n * sb, cudaMemcpyHostToDevice, s));
     }
     // (the first slice holds the level's head: kLevelHead <= 2^21 samples)
     if (off == 0 && (rc = launch_level(ctx, X, n_raw, sc, P, s))) return rc;
@@ -1042,17 +1014,17 @@ static int ingest_capture_host_impl(rfid_b200_ctx* ctx, const void* h_iq, bool s
   const int ns = *nseg;
   if (ns == 0) return RFID_B200_OK;
   const size_t res_bytes = (size_t)ns * max_windows_per_segment * sizeof(rfid_b200_window_result);
-  if ((rc = grow(ctx, &ctx->d_segs, &ctx->d_segs_bytes, (size_t)ns * sizeof(rfid_b200_segment)))) return rc;
-  if ((rc = grow(ctx, &ctx->d_res, &ctx->d_res_bytes, res_bytes))) return rc;
-  if ((rc = grow(ctx, &ctx->d_cnt, &ctx->d_cnt_bytes, (size_t)ns * 4))) return rc;
-  CK(cudaMemcpyAsync(ctx->d_segs, h_segs, (size_t)ns * sizeof(rfid_b200_segment), cudaMemcpyHostToDevice, s));
-  CK(cudaMemsetAsync(ctx->d_res, 0, res_bytes, s));
-  rc = decode_capture_impl(ctx, ctx->d_iq, sc16, scale, n_raw, (const rfid_b200_segment*)ctx->d_segs, ns,
-                           max_windows_per_segment, (rfid_b200_window_result*)ctx->d_res, (int32_t*)ctx->d_cnt, s, 0);
+  if ((rc = grow(ctx, ctx->d_segs, (size_t)ns * sizeof(rfid_b200_segment)))) return rc;
+  if ((rc = grow(ctx, ctx->d_res, res_bytes))) return rc;
+  if ((rc = grow(ctx, ctx->d_cnt, (size_t)ns * 4))) return rc;
+  CK(cudaMemcpyAsync(ctx->d_segs.p, h_segs, (size_t)ns * sizeof(rfid_b200_segment), cudaMemcpyHostToDevice, s));
+  CK(cudaMemsetAsync(ctx->d_res.p, 0, res_bytes, s));
+  rc = decode_capture_impl(ctx, ctx->d_iq.p, sc16, scale, n_raw, (const rfid_b200_segment*)ctx->d_segs.p, ns,
+                           max_windows_per_segment, (rfid_b200_window_result*)ctx->d_res.p, (int32_t*)ctx->d_cnt.p, s, 0);
   if (rc) return rc;
   ctx->last_launches += launches;
-  CK(cudaMemcpyAsync(h_results, ctx->d_res, res_bytes, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(h_counts, ctx->d_cnt, (size_t)ns * 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(h_results, ctx->d_res.p, res_bytes, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(h_counts, ctx->d_cnt.p, (size_t)ns * 4, cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
   return RFID_B200_OK;
 }
@@ -1183,9 +1155,9 @@ int rfid_b200_tx_synth(rfid_b200_ctx* ctx, const rfid_b200_tx_command* h_script,
   if (n_commands == 0) return RFID_B200_OK;
   CK(cudaSetDevice(ctx->device));
   const size_t sb = (size_t)n_commands * sizeof(rfid_b200_tx_command), ob = (size_t)n_commands * 8;
-  if ((rc = grow(ctx, &ctx->d_script, &ctx->d_script_bytes, sb + ob + 16))) return rc;
+  if ((rc = grow(ctx, ctx->d_script, sb + ob + 16))) return rc;
   cudaStream_t s = (cudaStream_t)stream;
-  unsigned long long* d_off = reinterpret_cast<unsigned long long*>(ctx->d_script);
+  unsigned long long* d_off = reinterpret_cast<unsigned long long*>(ctx->d_script.p);
   rfid_b200_tx_command* d_scr = reinterpret_cast<rfid_b200_tx_command*>(d_off + n_commands);
   // pageable sources: cudaMemcpyAsync stages them before returning, so the vectors may go out of scope
   CK(cudaMemcpyAsync(d_off, off.data(), ob, cudaMemcpyHostToDevice, s));
@@ -1247,18 +1219,18 @@ int rfid_b200_sim_capture(rfid_b200_ctx* ctx, const rfid_b200_sim_params* p, int
   } else {
     // Query + RN16 replies -> decode the RN16 window with this context's receive chain -> ACK(decoded) + EPC
     if (!pick_kernel(ctx->cfg)) { ctx->last_error = "capture mode supports decim = 5 only in this build"; return RFID_B200_EINVAL; }
-    if ((rc = grow(ctx, &ctx->d_sim_res, &ctx->d_sim_res_bytes, (size_t)nseg * sizeof(rfid_b200_window_result)))) return rc;
-    if ((rc = grow(ctx, &ctx->d_sim_cnt, &ctx->d_sim_cnt_bytes, (size_t)nseg * 4))) return rc;
+    if ((rc = grow(ctx, ctx->d_sim_res, (size_t)nseg * sizeof(rfid_b200_window_result)))) return rc;
+    if ((rc = grow(ctx, ctx->d_sim_cnt, (size_t)nseg * 4))) return rc;
     A.phase = 0;
     sim_slot_kernel<<<nseg, kSimThreads, smem, s>>>(A);
     CK(cudaGetLastError());
-    CK(cudaMemsetAsync(ctx->d_sim_res, 0, (size_t)nseg * sizeof(rfid_b200_window_result), s));
-    rc = rfid_b200_decode_capture(ctx, d_iq, (size_t)nseg * A.seg_len, d_segs, nseg, 1, (rfid_b200_window_result*)ctx->d_sim_res,
-                                  (int32_t*)ctx->d_sim_cnt, s);
+    CK(cudaMemsetAsync(ctx->d_sim_res.p, 0, (size_t)nseg * sizeof(rfid_b200_window_result), s));
+    rc = rfid_b200_decode_capture(ctx, d_iq, (size_t)nseg * A.seg_len, d_segs, nseg, 1, (rfid_b200_window_result*)ctx->d_sim_res.p,
+                                  (int32_t*)ctx->d_sim_cnt.p, s);
     if (rc) return rc;
     A.phase = 1;
-    A.rn16_records = (const rfid_b200_window_result*)ctx->d_sim_res;
-    A.rn16_counts = (const int32_t*)ctx->d_sim_cnt;
+    A.rn16_records = (const rfid_b200_window_result*)ctx->d_sim_res.p;
+    A.rn16_counts = (const int32_t*)ctx->d_sim_cnt.p;
     sim_slot_kernel<<<nseg, kSimThreads, smem, s>>>(A);
     CK(cudaGetLastError());
     launches = 3;
@@ -1343,19 +1315,19 @@ int rfid_b200_decode_commands_host(rfid_b200_ctx* ctx, const float* h_iq, size_t
   if (nseg == 0) return RFID_B200_OK;
   CK(cudaSetDevice(ctx->device));
   const size_t cmd_bytes = (size_t)nseg * max_commands_per_segment * sizeof(rfid_b200_command);
-  if ((rc = grow(ctx, &ctx->d_iq, &ctx->d_iq_bytes, n_raw * 8 + 16))) return rc;
-  if ((rc = grow(ctx, &ctx->d_segs, &ctx->d_segs_bytes, (size_t)nseg * sizeof(rfid_b200_segment)))) return rc;
-  if ((rc = grow(ctx, &ctx->d_cmd, &ctx->d_cmd_bytes, cmd_bytes))) return rc;
-  if ((rc = grow(ctx, &ctx->d_cnt, &ctx->d_cnt_bytes, (size_t)nseg * 4))) return rc;
+  if ((rc = grow(ctx, ctx->d_iq, n_raw * 8 + 16))) return rc;
+  if ((rc = grow(ctx, ctx->d_segs, (size_t)nseg * sizeof(rfid_b200_segment)))) return rc;
+  if ((rc = grow(ctx, ctx->d_cmd, cmd_bytes))) return rc;
+  if ((rc = grow(ctx, ctx->d_cnt, (size_t)nseg * 4))) return rc;
   cudaStream_t s = ctx->stream;
-  CK(cudaMemcpyAsync(ctx->d_iq, h_iq, n_raw * 8, cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(ctx->d_segs, h_segs, (size_t)nseg * sizeof(rfid_b200_segment), cudaMemcpyHostToDevice, s));
-  if (cmd_bytes) CK(cudaMemsetAsync(ctx->d_cmd, 0, cmd_bytes, s));
-  rc = decode_commands_impl(ctx, ctx->d_iq, false, 1.f, n_raw, (const rfid_b200_segment*)ctx->d_segs, nseg, cp,
-                            max_commands_per_segment, (rfid_b200_command*)ctx->d_cmd, (int32_t*)ctx->d_cnt, s);
+  CK(cudaMemcpyAsync(ctx->d_iq.p, h_iq, n_raw * 8, cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(ctx->d_segs.p, h_segs, (size_t)nseg * sizeof(rfid_b200_segment), cudaMemcpyHostToDevice, s));
+  if (cmd_bytes) CK(cudaMemsetAsync(ctx->d_cmd.p, 0, cmd_bytes, s));
+  rc = decode_commands_impl(ctx, ctx->d_iq.p, false, 1.f, n_raw, (const rfid_b200_segment*)ctx->d_segs.p, nseg, cp,
+                            max_commands_per_segment, (rfid_b200_command*)ctx->d_cmd.p, (int32_t*)ctx->d_cnt.p, s);
   if (rc) return rc;
-  if (cmd_bytes) CK(cudaMemcpyAsync(h_cmds, ctx->d_cmd, cmd_bytes, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(h_counts, ctx->d_cnt, (size_t)nseg * 4, cudaMemcpyDeviceToHost, s));
+  if (cmd_bytes) CK(cudaMemcpyAsync(h_cmds, ctx->d_cmd.p, cmd_bytes, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(h_counts, ctx->d_cnt.p, (size_t)nseg * 4, cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
   return RFID_B200_OK;
 }
@@ -1389,7 +1361,7 @@ int rfid_b200_window_quality(rfid_b200_ctx* ctx, const float* d_windows, const r
   A.empty_ratio = std::pow(10.0, (double)d.empty_db / 10.0);
   A.single_ratio = std::pow(10.0, (double)d.single_snr_db / 10.0);
   A.cfg = ctx->cfg;
-  rx_quality_kernel<<<(unsigned)((slots + kQualityWarps - 1) / kQualityWarps), 32 * kQualityWarps, 0, (cudaStream_t)stream>>>(A);
+  rx_quality_kernel<<<slot_grid(slots), 32 * kSlotWarps, 0, (cudaStream_t)stream>>>(A);
   CK(cudaGetLastError());
   ctx->last_launches = 1;
   return RFID_B200_OK;
@@ -1434,7 +1406,7 @@ int rfid_b200_recover_epc(rfid_b200_ctx* ctx, const float* d_windows, const rfid
   A.positions = d.positions; A.max_flips = d.max_flips; A.n_candidates = (int)n_candidates;
   A.min_snr_ratio = std::pow(10.0, (double)d.min_snr_db / 10.0);
   A.cfg = ctx->cfg;
-  rx_recover_kernel<<<(unsigned)((slots + kRecoverWarps - 1) / kRecoverWarps), 32 * kRecoverWarps, 0, (cudaStream_t)stream>>>(A);
+  rx_recover_kernel<<<slot_grid(slots), 32 * kSlotWarps, 0, (cudaStream_t)stream>>>(A);
   CK(cudaGetLastError());
   ctx->last_launches = 1;
   return RFID_B200_OK;
@@ -1474,8 +1446,8 @@ int rfid_b200_tag_report(rfid_b200_ctx* ctx, const rfid_b200_segment* d_segs, co
   const size_t agg_bytes = (size_t)slots * sizeof(ReportAgg), table_bytes = (size_t)buckets * 4;
   const size_t rep_bytes = (size_t)slots * 4, need = agg_bytes + table_bytes + rep_bytes + (size_t)n_blocks * 4;
   int rc;
-  if ((rc = grow(ctx, &ctx->d_report, &ctx->d_report_bytes, need))) return rc;
-  char* base = static_cast<char*>(ctx->d_report);
+  if ((rc = grow(ctx, ctx->d_report, need))) return rc;
+  char* base = static_cast<char*>(ctx->d_report.p);
   CK(cudaMemsetAsync(base, 0, agg_bytes + table_bytes, st));
   ReportArgs A;
   A.segs = d_segs; A.results = d_results; A.counts = d_counts; A.quality = d_quality; A.fix = d_fix;
@@ -1546,12 +1518,12 @@ int rfid_b200_match_epc(rfid_b200_ctx* ctx, const float* d_windows, const rfid_b
     // scratch: row count | rows [slots] (every attempted window is a row)
     const size_t need = 256 + (size_t)slots * sizeof(MatchRow);
     int rc;
-    if ((rc = grow(ctx, &ctx->d_match, &ctx->d_match_bytes, need))) return rc;
-    char* base = static_cast<char*>(ctx->d_match);
+    if ((rc = grow(ctx, ctx->d_match, need))) return rc;
+    char* base = static_cast<char*>(ctx->d_match.p);
     A.n_rows = reinterpret_cast<int32_t*>(base);
     A.rows = reinterpret_cast<MatchRow*>(base + 256);
     CK(cudaMemsetAsync(A.n_rows, 0, sizeof(int32_t), st));
-    rx_match_prepare_kernel<<<(unsigned)((slots + kMatchPrepWarps - 1) / kMatchPrepWarps), 32 * kMatchPrepWarps, 0, st>>>(A);
+    rx_match_prepare_kernel<<<slot_grid(slots), 32 * kSlotWarps, 0, st>>>(A);
     rx_match_score_kernel<<<(unsigned)((slots + kMatchRows - 1) / kMatchRows), 32 * kMatchWarps, 0, st>>>(A);
     launches += 2;
   }
@@ -1575,8 +1547,8 @@ int rfid_b200_gate_work(rfid_b200_ctx* ctx, int seek, const float* in, int n_in,
   // one device block [GateCallOut (64 B) | out: ns complex | |out|^2: ns floats] and its pinned host mirror: the kernel's
   // whole result comes back with ONE copy and ONE synchronisation per work call (it was two of each)
   const size_t off_out = 64, off_m2 = off_out + ns * 8, blk = off_m2 + ns * 4;
-  if ((rc = grow(ctx, &ctx->d_in, &ctx->d_in_bytes, ns * 8))) return rc;
-  if ((rc = grow(ctx, &ctx->d_blk, &ctx->d_blk_bytes, blk))) return rc;
+  if ((rc = grow(ctx, ctx->d_in, ns * 8))) return rc;
+  if ((rc = grow(ctx, ctx->d_blk, blk))) return rc;
   if (ctx->h_blk_bytes < blk) {
     if (ctx->h_blk) cudaFreeHost(ctx->h_blk);
     ctx->h_blk = nullptr; ctx->h_blk_bytes = 0;
@@ -1585,9 +1557,9 @@ int rfid_b200_gate_work(rfid_b200_ctx* ctx, int seek, const float* in, int n_in,
     ctx->h_blk_bytes = want;
   }
   cudaStream_t s = ctx->stream;
-  char* db = (char*)ctx->d_blk;
-  if (n_in) CK(cudaMemcpyAsync(ctx->d_in, in, (size_t)n_in * 8, cudaMemcpyHostToDevice, s));
-  gate_block_kernel<<<1, 32, 0, s>>>(ctx->cfg, ctx->d_gate, seek, (const float2*)ctx->d_in, n_in, (float2*)(db + off_out),
+  char* db = (char*)ctx->d_blk.p;
+  if (n_in) CK(cudaMemcpyAsync(ctx->d_in.p, in, (size_t)n_in * 8, cudaMemcpyHostToDevice, s));
+  gate_block_kernel<<<1, 32, 0, s>>>(ctx->cfg, (GateState*)ctx->d_gate.p, seek, (const float2*)ctx->d_in.p, n_in, (float2*)(db + off_out),
                                      (float*)(db + off_m2), (GateCallOut*)db);
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(ctx->h_blk, db, blk, cudaMemcpyDeviceToHost, s));
@@ -1612,13 +1584,13 @@ int rfid_b200_decoder_work(rfid_b200_ctx* ctx, int kind, const float* win, int n
   if (n < need) return RFID_B200_EINVAL;  // the reference only fires on a complete window (tag_decoder_impl.cc:223,291)
   CK(cudaSetDevice(ctx->device));
   int rc;
-  if ((rc = grow(ctx, &ctx->d_in, &ctx->d_in_bytes, (size_t)need * 8))) return rc;
+  if ((rc = grow(ctx, ctx->d_in, (size_t)need * 8))) return rc;
   cudaStream_t s = ctx->stream;
-  CK(cudaMemcpyAsync(ctx->d_in, win, (size_t)need * 8, cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(ctx->d_in.p, win, (size_t)need * 8, cudaMemcpyHostToDevice, s));
   const int stage = chunk_stage_samples(ctx->cfg);
-  decode_block_kernel<<<1, 32, (size_t)stage * 8, s>>>(ctx->cfg, kind, (const float2*)ctx->d_in, need, stage, ctx->d_one);
+  decode_block_kernel<<<1, 32, (size_t)stage * 8, s>>>(ctx->cfg, kind, (const float2*)ctx->d_in.p, need, stage, (rfid_b200_window_result*)ctx->d_one.p);
   CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(res, ctx->d_one, sizeof(*res), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(res, ctx->d_one.p, sizeof(*res), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
   if (bits_out) {
     const int nb = kind == RFID_B200_RN16 ? 16 : 128;
@@ -1641,17 +1613,17 @@ int rfid_b200_mf_work(rfid_b200_ctx* ctx, const float* in, int n_in, float* out,
   int rc;
   const size_t total = (size_t)(ctx->mf_have + n_in);
   // staging buffer = carried history + new chunk
-  if ((rc = grow(ctx, &ctx->d_out, &ctx->d_out_bytes, (total + 1) * 8))) return rc;
+  if ((rc = grow(ctx, ctx->d_out, (total + 1) * 8))) return rc;
   cudaStream_t s = ctx->stream;
-  if (ctx->mf_have) CK(cudaMemcpyAsync(ctx->d_out, ctx->d_mf, (size_t)ctx->mf_have * 8, cudaMemcpyDeviceToDevice, s));
-  if (n_in) CK(cudaMemcpyAsync((char*)ctx->d_out + (size_t)ctx->mf_have * 8, in, (size_t)n_in * 8, cudaMemcpyHostToDevice, s));
+  if (ctx->mf_have) CK(cudaMemcpyAsync(ctx->d_out.p, ctx->d_mf.p, (size_t)ctx->mf_have * 8, cudaMemcpyDeviceToDevice, s));
+  if (n_in) CK(cudaMemcpyAsync((char*)ctx->d_out.p + (size_t)ctx->mf_have * 8, in, (size_t)n_in * 8, cudaMemcpyHostToDevice, s));
   if (n_out > 0) {
-    if ((rc = grow(ctx, &ctx->d_m2, &ctx->d_m2_bytes, (size_t)n_out * 8))) return rc;
+    if ((rc = grow(ctx, ctx->d_m2, (size_t)n_out * 8))) return rc;
     const int threads = 128;
     mf_block_kernel<<<(unsigned)((n_out + threads - 1) / threads), threads, 0, s>>>(
-        ctx->cfg, (const float2*)ctx->d_out, ctx->mf_abs0, ctx->mf_next_n, (int)n_out, (float2*)ctx->d_m2);
+        ctx->cfg, (const float2*)ctx->d_out.p, ctx->mf_abs0, ctx->mf_next_n, (int)n_out, (float2*)ctx->d_m2.p);
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(out, ctx->d_m2, (size_t)n_out * 8, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(out, ctx->d_m2.p, (size_t)n_out * 8, cudaMemcpyDeviceToHost, s));
   }
   // keep what the next output still needs: samples from D*next_n - (K-1) on
   const long long next_n = ctx->mf_next_n + n_out;
@@ -1659,8 +1631,8 @@ int rfid_b200_mf_work(rfid_b200_ctx* ctx, const float* in, int n_in, float* out,
   if (keep_from < ctx->mf_abs0) keep_from = ctx->mf_abs0;
   if (keep_from > abs_end) keep_from = abs_end;
   const long long keep = abs_end - keep_from;
-  if ((rc = grow(ctx, &ctx->d_mf, &ctx->d_mf_bytes, (size_t)(keep + 1) * 8))) return rc;
-  if (keep) CK(cudaMemcpyAsync(ctx->d_mf, (char*)ctx->d_out + (size_t)(keep_from - ctx->mf_abs0) * 8, (size_t)keep * 8,
+  if ((rc = grow(ctx, ctx->d_mf, (size_t)(keep + 1) * 8))) return rc;
+  if (keep) CK(cudaMemcpyAsync(ctx->d_mf.p, (char*)ctx->d_out.p + (size_t)(keep_from - ctx->mf_abs0) * 8, (size_t)keep * 8,
                                cudaMemcpyDeviceToDevice, s));
   CK(cudaStreamSynchronize(s));
   ctx->mf_abs0 = keep_from; ctx->mf_have = keep; ctx->mf_next_n = next_n;

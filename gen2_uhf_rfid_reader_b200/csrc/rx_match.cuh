@@ -16,7 +16,6 @@
 
 namespace rfid_b200 {
 
-constexpr int kMatchPrepWarps = 4;                  // prepare: warps (= record slots) per CTA
 constexpr int kMatchWarps = 4;                      // score: warps per CTA
 constexpr int kMatchWarpRows = 32;                  // rows per warp (two m16 tiles)
 constexpr int kMatchRows = kMatchWarps * kMatchWarpRows;
@@ -88,14 +87,13 @@ __global__ void rx_match_init_kernel(const MatchArgs A)
   if (e < A.max_dict) reinterpret_cast<int4*>(A.match_count)[e] = make_int4(0, -1, -1, 0);
 }
 
-__global__ void __launch_bounds__(32 * kMatchPrepWarps) rx_match_prepare_kernel(const MatchArgs A)
+__global__ void __launch_bounds__(32 * kSlotWarps) rx_match_prepare_kernel(const MatchArgs A)
 {
   const int lane = threadIdx.x & 31;
-  const long long slot = (long long)blockIdx.x * kMatchPrepWarps + (threadIdx.x >> 5);
-  if (slot >= (long long)A.nseg * A.max_windows) return;
-  const int seg = (int)(slot / A.max_windows), k = (int)(slot % A.max_windows);
-  if (k >= min(A.counts[seg], A.max_windows)) return;
-  const rfid_b200_window_result& rec = A.results[slot];
+  TapWindow t;
+  if (!tap_window(A, t)) return;
+  const long long slot = t.slot;
+  const rfid_b200_window_result& rec = *t.rec;
   rfid_b200_epc_match* out = A.match + slot;
   if (rec.kind != RFID_B200_EPC || rec.crc_ok == 1 || (A.fix && A.fix[slot].status == RFID_B200_FIX_RECOVERED)) {
     if (lane == 0)
@@ -106,17 +104,11 @@ __global__ void __launch_bounds__(32 * kMatchPrepWarps) rx_match_prepare_kernel(
     if (lane == 0) match_store(out, RFID_B200_MATCH_SKIPPED, -1, -1, -1, -1);
     return;
   }
-  const RxConfig& c = A.cfg;
-  const float2* w = A.windows + slot * c.len_epc;
-  const int n = max(0, min(rec.length, c.len_epc));
-  const int index = win_data_index(c, rec.sync_index);
-  const float2 h = make_float2(rec.h_re, rec.h_im);
-  const float T = rec.T, twoT = f_mul(2.0f, T);
   float r[4];
   double a1 = 0.0;
 #pragma unroll
   for (int i = 0; i < 4; i++) {   // lane l holds decisions j = 32 i + l
-    r[i] = epc_projection(w, n, i * 32 + lane, T, twoT, index, h);
+    r[i] = epc_projection(t, i * 32 + lane);
     a1 = __dadd_rn(a1, (double)fabsf(r[i]));
   }
   const double s1 = quality_lane_sum(a1);

@@ -9,7 +9,6 @@
 
 namespace rfid_b200 {
 
-constexpr int kRecoverWarps = 4;                 // warps (= record slots) per CTA
 constexpr int kRecoverMaxPositions = 32;         // P: one candidate position per lane
 constexpr long long kRecoverMaxCandidates = 65536;
 
@@ -89,27 +88,25 @@ __device__ __forceinline__ void recover_store(rfid_b200_epc_fix* out, int status
   o[1] = make_int4((int)mem[0], (int)mem[1], (int)mem[2], (int)mem[3]);
 }
 
-__global__ void __launch_bounds__(32 * kRecoverWarps) rx_recover_kernel(const RecoverArgs A)
+__global__ void __launch_bounds__(32 * kSlotWarps) rx_recover_kernel(const RecoverArgs A)
 {
-  __shared__ uint32_t s_col[kRecoverWarps][kRecoverMaxPositions];
+  __shared__ uint32_t s_col[kSlotWarps][kRecoverMaxPositions];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const long long slot = (long long)blockIdx.x * kRecoverWarps + warp;
-  if (slot >= (long long)A.nseg * A.max_windows) return;
-  const int seg = (int)(slot / A.max_windows), k = (int)(slot % A.max_windows);
-  if (k >= min(A.counts[seg], A.max_windows)) return;
-  const rfid_b200_window_result& rec = A.results[slot];
+  TapWindow t;
+  if (!tap_window(A, t)) return;
+  const rfid_b200_window_result& rec = *t.rec;
   const float nan = __int_as_float(0x7fc00000);
   uint32_t mem[4];   // the record's 16 bytes as 4 little-endian words
   {
     const uint4 b = *reinterpret_cast<const uint4*>(rec.bits);
     mem[0] = b.x; mem[1] = b.y; mem[2] = b.z; mem[3] = b.w;
   }
-  rfid_b200_epc_fix* out = A.fix + slot;
+  rfid_b200_epc_fix* out = A.fix + t.slot;
   if (rec.kind != RFID_B200_EPC || rec.crc_ok == 1) {
     if (lane == 0) recover_store(out, rec.kind != RFID_B200_EPC ? RFID_B200_FIX_NOT_EPC : RFID_B200_FIX_CRC_OK, 0, 0, nan, mem);
     return;
   }
-  const rfid_b200_quality q = A.quality[slot];
+  const rfid_b200_quality q = A.quality[t.slot];
   if (!(q.n_decisions == 128 && (double)q.snr >= A.min_snr_ratio)) {
     if (lane == 0) recover_store(out, RFID_B200_FIX_SKIPPED, 0, 0, nan, mem);
     return;
@@ -118,18 +115,12 @@ __global__ void __launch_bounds__(32 * kRecoverWarps) rx_recover_kernel(const Re
   uint32_t word[4];   // bit j at word[j >> 5], bit j & 31
 #pragma unroll
   for (int i = 0; i < 4; i++) word[i] = __brev(__byte_perm(mem[i], 0, 0x0123));
-  const RxConfig& c = A.cfg;
-  const float2* w = A.windows + slot * c.len_epc;
-  const int n = max(0, min(rec.length, c.len_epc));
-  const int index = win_data_index(c, rec.sync_index);
-  const float2 h = make_float2(rec.h_re, rec.h_im);
-  const float T = rec.T, twoT = f_mul(2.0f, T);
   float rho[4];
   uint32_t syn = 0u;
 #pragma unroll
   for (int i = 0; i < 4; i++) {
     const int j = i * 32 + lane;
-    rho[i] = fabsf(epc_projection(w, n, j, T, twoT, index, h));
+    rho[i] = fabsf(epc_projection(t, j));
     if ((word[i] >> lane) & 1u) syn ^= kEpcSyndrome.col[j];
   }
 #pragma unroll
